@@ -92,6 +92,11 @@ PHASTFT_API int32_t phastft_plan_dit_f32_reserve(const phastft_plan_dit_f32* pla
  * planner uses for `num_points` (one CTA per transform when *num_passes == 1; 0 passes for N == 1).
  * log2_factors must hold 3 ints. */
 PHASTFT_API int32_t phastft_plan_factorization(size_t num_points, int precision_bits, int* log2_factors, int* num_passes);
+/* Host-only: the alternative plans PHASTFT_MODE_TUNE times against the heuristic one for `num_points` (the tuner reads
+ * this same list).  Candidate i has the pass sizes 2^log2_factors[3i + p] and tile widths pass_c[3i + p] (columns) for
+ * p < its number of passes; unused slots are 0.  *count receives the number of candidates (0 for one-CTA sizes); at most
+ * `max` are written. */
+PHASTFT_API int32_t phastft_plan_tune_candidates(size_t num_points, int precision_bits, int* log2_factors, int* pass_c, int max, int* count);
 
 /* Planner-table blob (multi-GPU init, SURVEY.md section 8e): rank 0 exports its tables into a
  * device buffer, the host framework broadcasts that buffer once (ncclBroadcast /

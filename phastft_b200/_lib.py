@@ -125,7 +125,26 @@ def plan_factorization(n: int, precision_bits: int = 64):
     return [f[i] for i in range(k.value)]
 
 
-GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_device_count",
+lib.phastft_plan_tune_candidates.argtypes = [_sz, _ci, C.POINTER(_ci), C.POINTER(_ci), _ci, C.POINTER(_ci)]
+lib.phastft_plan_tune_candidates.restype = _i32
+
+
+def plan_tune_candidates(n: int, precision_bits: int = 64):
+    """Host-only: the plans PlannerMode::Tune times for an n-point transform, as (log2 pass sizes, tile columns) pairs."""
+    k = _ci(0)
+    check(lib.phastft_plan_tune_candidates(int(n), int(precision_bits), None, None, 0, C.byref(k)))
+    f = (_ci * (3 * k.value))()
+    c = (_ci * (3 * k.value))()
+    check(lib.phastft_plan_tune_candidates(int(n), int(precision_bits), f, c, k.value, C.byref(k)))
+    out = []
+    for i in range(k.value):
+        used = [p for p in range(3) if f[3 * i + p]]
+        out.append(([f[3 * i + p] for p in used], [c[3 * i + p] for p in used]))
+    return out
+
+
+GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization",
+                  "phastft_plan_tune_candidates", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_device_count",
                   "phastft_options_default", "phastft_options_guess"]
 
 for _name, (_args, _res) in SIGNATURES.items():

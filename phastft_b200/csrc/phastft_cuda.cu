@@ -1572,6 +1572,43 @@ int32_t batch_sharded_host(Plan<T>* const* plans, int num_plans, T* re, T* im, s
 // the reference accepts the mode and ignores it, planner.rs:65).  Here it is real: a handful of pass
 // decompositions / tile widths around the heuristic choice are built, timed on a scratch signal with CUDA
 // events, and the fastest is kept.
+//
+// The candidates, host-only (phastft_plan_tune_candidates exposes the same list, so tests can force every plan the
+// tuner may pick).  Each entry is stated as it builds: strided tiles exist for 32..1024 rows, a 1024-row tile has no
+// CW build (CN is the widest), and the 1024-row middle pass of a 3-pass plan is the half-width CH tile (id 62).
+template <typename T>
+std::vector<PlanChoice> tune_candidates(int ln) {
+    std::vector<PlanChoice> cands;
+    if (ln == 0 || choose_factors<T>(ln).size() < 2) return cands;    // one-CTA sizes: nothing to choose
+    const int CH = TileC<T>::CH, CN = TileC<T>::CN, CW = TileC<T>::CW;
+    auto width = [&](int log2r, int c) { return log2r == 10 ? std::min(c, CN) : c; };
+    auto add = [&](std::vector<int> f, std::vector<int> c) {
+        for (size_t p = 0; p < f.size(); ++p) c[p] = width(f[p], c[p]);
+        if (f.size() == 3 && f[1] == 10) c[1] = CH;
+        for (const PlanChoice& q : cands)
+            if (q.factors == f && q.pass_c == c) return;
+        PlanChoice pc; pc.factors = std::move(f); pc.pass_c = std::move(c); cands.push_back(std::move(pc));
+    };
+    if (ln <= 20) {
+        for (int a : {ln / 2, (ln + 1) / 2})
+            for (int c : {CH, CN, CW}) {
+                if (a > 10 || ln - a > 10 || a < 5 || ln - a < 5) continue;
+                add({a, ln - a}, {c, c});
+            }
+        if (ln >= 18) add({6, ln - 12, 6}, {CN, CN, CN});
+        if (ln >= 19) add({7, ln - 14, 7}, {CN, CN, CN});
+    } else {
+        for (int e : {7, 8, 9}) {
+            const int m = ln - 2 * e;
+            if (m < 5 || m > 10) continue;
+            add({e, m, e}, {CW, CN, CW});
+            add({e, m, e}, {CN, CN, CN});
+        }
+        if (ln - 18 >= 5 && ln - 18 <= 10) { add({10, ln - 18, 8}, {CN, CN, CW}); add({8, ln - 18, 10}, {CW, CN, CN}); }
+    }
+    return cands;
+}
+
 template <typename T>
 int32_t build_plan_tuned(size_t n, int device, Plan<T>** out) {
     if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
@@ -1582,25 +1619,7 @@ int32_t build_plan_tuned(size_t n, int device, Plan<T>** out) {
     const int ln = best->log2n;
     if (best->num_passes < 2) return PHASTFT_OK;            // one-CTA sizes: nothing to choose
     DeviceGuard guard(device);
-    const int CH = TileC<T>::CH, CN = TileC<T>::CN, CW = TileC<T>::CW;
-    std::vector<PlanChoice> cands;
-    auto add = [&](std::vector<int> f, std::vector<int> c) { PlanChoice pc; pc.factors = std::move(f); pc.pass_c = std::move(c); cands.push_back(std::move(pc)); };
-    if (ln <= 20) {
-        for (int a : {ln / 2, (ln + 1) / 2})
-            for (int c : {CH, CN, CW}) {
-                if (a > 10 || ln - a > 10 || a < 5 || ln - a < 5) continue;
-                add({a, ln - a}, {c, c});
-            }
-        if (ln >= 18) { add({6, ln - 12, 6}, {CN, CN, CN}); add({7, ln - 14, 7}, {CN, CN, CN}); }
-    } else {
-        for (int e : {7, 8, 9}) {
-            const int m = ln - 2 * e;
-            if (m < 5 || m > 10) continue;
-            add({e, m, e}, {CW, CN, CW});
-            add({e, m, e}, {CN, CN, CN});
-        }
-        if (ln - 18 >= 5 && ln - 18 <= 10) { add({10, ln - 18, 8}, {CN, CN, CW}); add({8, ln - 18, 10}, {CW, CN, CN}); }
-    }
+    const std::vector<PlanChoice> cands = tune_candidates<T>(ln);
     T *re = nullptr, *im = nullptr;
     if (cudaMalloc(&re, n * sizeof(T)) != cudaSuccess || cudaMalloc(&im, n * sizeof(T)) != cudaSuccess) {
         cudaGetLastError();
@@ -1995,6 +2014,22 @@ int32_t phastft_plan_factorization(size_t n, int precision_bits, int* log2_facto
     std::vector<int> f = ln == 0 ? std::vector<int>{} : (precision_bits == 64 ? choose_factors<double>(ln) : choose_factors<float>(ln));
     *num_passes = (int)f.size();
     for (size_t i = 0; i < f.size(); ++i) log2_factors[i] = f[i];
+    return PHASTFT_OK;
+}
+
+int32_t phastft_plan_tune_candidates(size_t n, int precision_bits, int* log2_factors, int* pass_c, int max, int* count) {
+    if (!count || (max > 0 && (!log2_factors || !pass_c))) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
+    if (!is_pow2(n)) return fail(PHASTFT_ERR_NOT_POW2);
+    if (precision_bits != 32 && precision_bits != 64) return fail(PHASTFT_ERR_INVALID_ARG, "precision_bits must be 32 or 64");
+    const int ln = ilog2(n);
+    const std::vector<PlanChoice> c = precision_bits == 64 ? tune_candidates<double>(ln) : tune_candidates<float>(ln);
+    *count = (int)c.size();
+    for (int i = 0; i < std::min(max, (int)c.size()); ++i)
+        for (int p = 0; p < MAX_PASSES; ++p) {
+            const bool used = p < (int)c[i].factors.size();
+            log2_factors[MAX_PASSES * i + p] = used ? c[i].factors[p] : 0;
+            pass_c[MAX_PASSES * i + p] = used ? c[i].pass_c[p] : 0;
+        }
     return PHASTFT_OK;
 }
 

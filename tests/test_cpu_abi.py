@@ -117,6 +117,27 @@ def test_planner_factorization_host_logic(pf):
         _lib.plan_factorization(12, 64)
 
 
+def test_tune_candidates_host_logic(pf):
+    """The plans PlannerMode::Tune times: host-only, none for one-CTA sizes, every one a valid decomposition whose tiles exist
+    as listed (no 1024-row tile wider than CN; the 1024-row middle pass of a 3-pass plan is the half-width CH tile)."""
+    from phastft_b200 import _lib
+    for bits, single_max, (ch, cn, cw) in ((64, 11, (4, 8, 16)), (32, 13, (8, 16, 32))):
+        for ln in range(0, 31):
+            cands = _lib.plan_tune_candidates(1 << ln, bits)
+            if ln <= single_max or ln >= 29:
+                assert cands == [], (bits, ln, cands)
+                continue
+            assert cands, (bits, ln)
+            assert len({(tuple(f), tuple(c)) for f, c in cands}) == len(cands)        # no duplicates
+            for f, c in cands:
+                assert sum(f) == ln and len(f) == len(c) in (2, 3) and all(5 <= x <= 10 for x in f), (ln, f)
+                assert all(w in (ch, cn, cw) for w in c) and all(w <= cn for x, w in zip(f, c) if x == 10), (ln, f, c)
+                if len(f) == 3 and f[1] == 10:
+                    assert c[1] == ch
+    with pytest.raises(pf.PhastFTPanic):
+        _lib.plan_tune_candidates(12, 64)
+
+
 def test_rust_ffi_is_generated_from_the_header():
     """rust/src/ffi.rs binds every PHASTFT_API declaration: it is the output of tools/gen_rust_ffi.py on the current header."""
     import importlib.util

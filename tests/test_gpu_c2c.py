@@ -10,6 +10,8 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import truth
+
 pytestmark = pytest.mark.gpu
 
 GOLD = Path(__file__).resolve().parent / "golden"
@@ -68,11 +70,10 @@ def test_forward_and_reverse_vs_oracle(dt, log_n):
         O.fft_dit(o_re, o_im, odir)
         err = rel_linf(g_re, g_im, o_re, o_im)
         assert err <= tol(dt, n), (planner.describe(), direction, err)
-    # independent truth as well (numpy pocketfft, f64)
-    truth = np.fft.fft(re0.astype(np.float64) + 1j * im0.astype(np.float64))
+    # independent truth as well (long double, tests/truth.py bounds)
     g_re, g_im = re0.copy(), im0.copy()
     fft_with_planner(dt)(g_re, g_im, pf.Direction.Forward, planner)
-    assert rel_linf(g_re, g_im, truth.real, truth.imag) <= tol(dt, n)
+    truth.check(g_re, g_im, truth.fft_ld(re0, im0), dt, n, "oracle-seeded fwd")
 
 
 # --- committed golden vectors; the GPU must be at least as close to the truth as ~2x the oracle --
@@ -325,7 +326,7 @@ def test_config_batch_f32_2pow16_linearity_and_oracle():
 # --- PlannerMode::Tune is real here: it must stay correct and never be slower than the heuristic plan ----
 @pytest.mark.parametrize("dt", [np.float64, np.float32])
 @pytest.mark.parametrize("log_n", [14, 18, 22])
-def test_tune_mode_correct_and_not_slower(dt, log_n):
+def test_tune_mode_correct_and_not_slower(dt, log_n, monkeypatch):
     import torch
     pf, O = _pf(), _O()
     n = 1 << log_n
@@ -333,6 +334,14 @@ def test_tune_mode_correct_and_not_slower(dt, log_n):
     tuned = P.with_mode(n, pf.PlannerMode.Tune)
     plain = P(n)
     assert tuned.describe().endswith("[tuned]")
+    # the tuner picked the heuristic plan or one of its listed candidates (forced here one by one)
+    known = {plain.describe()}
+    with monkeypatch.context() as m:
+        for factors, widths in pf._lib.plan_tune_candidates(n, 64 if dt == np.float64 else 32):
+            m.setenv("PHASTFT_FACTORS", f"{log_n}:" + ",".join(map(str, factors)))
+            m.setenv("PHASTFT_PASS_C", ",".join(map(str, widths)))
+            known.add(P(n).describe())
+    assert tuned.describe()[: -len(" [tuned]")] in known, tuned.describe()
     re0, im0 = O.gen_random_signal(n, dt, seed=log_n)
     g_re, g_im = re0.copy(), im0.copy()
     fft_with_planner(dt)(g_re, g_im, pf.Direction.Forward, tuned)

@@ -3,13 +3,15 @@
 Tolerance: the reference builds its w[k] = 0.5 W_N^k table by an O(N) rotation recurrence
 (planner.rs:128-138) whose error grows with N (6e-12 at 2^20 in f64); the GPU looks the same
 twiddles up exactly.  So parity is stated against BOTH references:
-  vs numpy.fft.rfft (f64 truth):  rel-Linf <= 4 * eps * log2(N)
-  vs the oracle:                  rel-Linf <= 4 * eps * log2(N) + (oracle's own error vs truth)
+  vs the long-double rfft (tests/truth.py):  the bounds of tests/truth.py (C * eps * sqrt(log2 N), L-inf and RMS)
+  vs the oracle:                             rel-Linf <= 4 * eps * log2(N) + (oracle's own error vs truth)
 """
 from pathlib import Path
 
 import numpy as np
 import pytest
+
+import truth as TR
 
 pytestmark = pytest.mark.gpu
 GOLD = Path(__file__).resolve().parent / "golden"
@@ -50,13 +52,12 @@ def test_r2c_c2r_vs_truth_and_oracle(dt, log_n):
     planner = P(n)
     g_re = np.zeros(half + 1, dt); g_im = np.zeros(half + 1, dt)
     r2c_p(x, g_re, g_im, planner)
-    truth = np.fft.rfft(x.astype(np.float64))
+    truth = TR.rfft_ld(x)
     o_re = np.zeros(half + 1, dt); o_im = np.zeros(half + 1, dt)
     O.r2c_fft(x, o_re, o_im)
     G = g_re.astype(np.float64) + 1j * g_im
     Oc = o_re.astype(np.float64) + 1j * o_im
-    e_truth = rel(G, truth)
-    assert e_truth <= tol(dt, n), e_truth
+    TR.check(g_re, g_im, truth, dt, n, "r2c")
     assert rel(G, Oc) <= tol(dt, n) + rel(Oc, truth)
     assert g_im[0] == 0 and g_im[half] == 0                       # r2c.rs:161-166
     # c2r of the GPU spectrum restores x (fully normalised)
@@ -201,9 +202,7 @@ def test_config_r2c_2pow24_roundtrip_device():
     d_x = torch.from_numpy(x).cuda()
     d_re = torch.empty(half + 1, dtype=torch.float64, device="cuda"); d_im = torch.empty_like(d_re)
     pf.r2c_fft_f64_with_planner(d_x, d_re, d_im, pl)
-    truth = np.fft.rfft(x)
-    G = d_re.cpu().numpy() + 1j * d_im.cpu().numpy()
-    assert rel(G, truth) <= tol(np.float64, n)
+    TR.check(d_re.cpu().numpy(), d_im.cpu().numpy(), TR.rfft_ld(x), np.float64, n, "r2c")
     d_y = torch.empty(n, dtype=torch.float64, device="cuda")
     s_re = torch.empty(half, dtype=torch.float64, device="cuda"); s_im = torch.empty_like(s_re)
     pf.c2r_fft_f64_with_planner_and_scratch(d_re, d_im, d_y, pl, s_re, s_im)
@@ -243,5 +242,4 @@ def test_c2r_preprocessing_on_load_matches_separate_sweep(dt, log_n, monkeypatch
     y = torch.empty(n, dtype=tdt, device="cuda")
     c2r_p(d_re, d_im, y, pl)
     if log_n <= 22:
-        truth = np.fft.irfft(d_re.cpu().numpy().astype(np.float64) + 1j * d_im.cpu().numpy().astype(np.float64), n)
-        assert np.max(np.abs(y.cpu().numpy() - truth)) <= tol(dt, n) * max(np.max(np.abs(truth)), 1.0) * 4
+        TR.check(y.cpu().numpy(), None, TR.irfft_ld(d_re.cpu().numpy(), d_im.cpu().numpy(), n), dt, n, "c2r fused")
