@@ -41,6 +41,15 @@ PHASTFT_API const char* phastft_version(void);
 PHASTFT_API int32_t phastft_device_count(int* count);
 /* number of CUDA kernels this library has launched in this process (bench.py "gpu_launches") */
 PHASTFT_API uint64_t phastft_launch_count(void);
+/* Thread-local, like phastft_last_error: the kernels the calling thread's most recent execution call (any *_host,
+ * *_oneshot, *_dev, *_dev_profile or *_batch_sharded_host entry point) launched, one entry per launch, in order, separated
+ * by "; ".  Each entry reads "<kind> R=<rows> C=<columns> NT=<threads> v<variant> <mode>[ pdl]": kind COL / TRANS (strided
+ * passes), ROW (one CTA per transform), CLUSTER (both passes in one cluster launch: R=<R1>x<R2>, K=<CTAs per cluster>),
+ * PIPE (both passes in one pipelined launch: R=<R1>x<R2>), R2C-UNTANGLE / C2R-PRE (the real transforms' elementwise
+ * kernels); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
+ * Reset at the start of every execution call; valid until the thread's next call. */
+PHASTFT_API const char* phastft_last_launches(void);
 /* The *_oneshot entry points (a planner per call, lib.rs:180 / r2c.rs:522,696) keep their most recent plan per
  * precision and reuse it when the next call has the same size and device; this releases those plans and their
  * device buffers. */
@@ -180,7 +189,9 @@ PHASTFT_API int32_t phastft_r2c_f64_oneshot(const double* input, size_t len_in, 
                                             double* output_im, size_t len_oim, int device);
 PHASTFT_API int32_t phastft_r2c_f32_oneshot(const float* input, size_t len_in, float* output_re, size_t len_ore,
                                             float* output_im, size_t len_oim, int device);
-/* Device-resident: d_input N reals, d_out_re/d_out_im N/2+1 each; asynchronous on `stream`. */
+/* Device-resident: d_input N reals, d_out_re/d_out_im N/2+1 each; asynchronous on `stream`.
+ * d_input is read as N/2 (re, im) pairs: it must be aligned to 2 * sizeof(T) bytes (16 for f64, 8 for f32), else
+ * PHASTFT_ERR_INVALID_ARG and nothing is launched. */
 PHASTFT_API int32_t phastft_r2c_f64_dev(const phastft_plan_r2c_f64* plan, const double* d_input, double* d_out_re,
                                         double* d_out_im, void* stream);
 PHASTFT_API int32_t phastft_r2c_f32_dev(const phastft_plan_r2c_f32* plan, const float* d_input, float* d_out_re,
@@ -202,7 +213,8 @@ PHASTFT_API int32_t phastft_c2r_f64_oneshot(const double* input_re, size_t len_i
                                             size_t len_iim, double* output, size_t len_out, int device);
 PHASTFT_API int32_t phastft_c2r_f32_oneshot(const float* input_re, size_t len_ire, const float* input_im,
                                             size_t len_iim, float* output, size_t len_out, int device);
-/* Device-resident: d_scratch_re/d_scratch_im N/2 each or both NULL (plan workspace). */
+/* Device-resident: d_scratch_re/d_scratch_im N/2 each or both NULL (plan workspace).  d_output is written as N/2
+ * (re, im) pairs: it must be aligned to 2 * sizeof(T) bytes, else PHASTFT_ERR_INVALID_ARG and nothing is launched. */
 PHASTFT_API int32_t phastft_c2r_f64_dev(const phastft_plan_r2c_f64* plan, const double* d_in_re, const double* d_in_im,
                                         double* d_output, double* d_scratch_re, double* d_scratch_im, void* stream);
 PHASTFT_API int32_t phastft_c2r_f32_dev(const phastft_plan_r2c_f32* plan, const float* d_in_re, const float* d_in_im,
@@ -212,7 +224,8 @@ PHASTFT_API int32_t phastft_c2r_f32_dev(const phastft_plan_r2c_f32* plan, const 
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The
  * reference deinterleaves into two fresh Vecs, runs the planar FFT and re-interleaves
  * (complex_nums.rs:11-55); here the AoS<->planar conversion is fused into the first pass's
- * load and the last pass's store. */
+ * load and the last pass's store.  The *_dev form accesses d_signal as (re, im) pairs: it must be aligned to
+ * 2 * sizeof(T) bytes (a Complex<T>'s own alignment), else PHASTFT_ERR_INVALID_ARG and nothing is launched. */
 PHASTFT_API int32_t phastft_fft_interleaved_f64_host(const phastft_plan_dit_f64* plan, double* signal, size_t len_complex,
                                                      int direction);
 PHASTFT_API int32_t phastft_fft_interleaved_f32_host(const phastft_plan_dit_f32* plan, float* signal, size_t len_complex,

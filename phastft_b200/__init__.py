@@ -5,4 +5,4 @@ libphastft_cuda.so (csrc/, include/phastft_cuda.h).  Importing it requires the b
 library; there is no CPU fallback.
 """
 from .api import *  # noqa: F401,F403
-from ._lib import LIB_PATH, device_count, launch_count  # noqa: F401
+from ._lib import LIB_PATH, device_count, last_launches, launch_count  # noqa: F401

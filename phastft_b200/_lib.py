@@ -62,6 +62,7 @@ _sz, _vp, _i32, _ci = C.c_size_t, C.c_void_p, C.c_int32, C.c_int
 lib.phastft_last_error.restype = C.c_char_p
 lib.phastft_version.restype = C.c_char_p
 lib.phastft_launch_count.restype = C.c_uint64
+lib.phastft_last_launches.restype = C.c_char_p
 lib.phastft_device_count.argtypes = [C.POINTER(_ci)]
 lib.phastft_device_count.restype = _i32
 
@@ -144,8 +145,8 @@ def plan_tune_candidates(n: int, precision_bits: int = 64):
 
 
 GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization",
-                  "phastft_plan_tune_candidates", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_device_count",
-                  "phastft_options_default", "phastft_options_guess"]
+                  "phastft_plan_tune_candidates", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
+                  "phastft_device_count", "phastft_options_default", "phastft_options_guess"]
 
 for _name, (_args, _res) in SIGNATURES.items():
     for _s in ("f64", "f32"):
@@ -162,6 +163,12 @@ def fn(name: str, sfx: str):
 
 def launch_count() -> int:
     return int(lib.phastft_launch_count())
+
+
+def last_launches() -> list:
+    """The kernels this thread's most recent library call launched, one string per launch (include/phastft_cuda.h)."""
+    text = (lib.phastft_last_launches() or b"").decode()
+    return text.split("; ") if text else []
 
 
 def device_count() -> int:

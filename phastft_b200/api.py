@@ -95,6 +95,12 @@ def _torch_ptr(t, dtype):
     return C.c_void_p(t.data_ptr()), t.numel()
 
 
+def _pair_aligned(t) -> bool:
+    """r2c reads its real input and c2r writes its real output as (re, im) pairs, so those device pointers must be aligned
+    to 2 * sizeof(T); a view of a real tensor can start at any element, e.g. x[1:]."""
+    return t.data_ptr() % (2 * t.element_size()) == 0
+
+
 def _torch_stream(t):
     import torch
     return C.c_void_p(torch.cuda.current_stream(t.device).cuda_stream)
@@ -363,6 +369,7 @@ def _interleaved(sfx, dtype, cdtype, signal, direction, planner):
             raise PhastFTPanic(2)
         if n != planner.num_points:
             raise PhastFTPanic(3)
+        # (torch keeps a complex tensor's storage offset in whole elements, so its pointer is pair-aligned)
         check(fn("phastft_fft_interleaved_{s}_dev", sfx)(planner._h, C.c_void_p(signal.data_ptr()), int(direction), 1, n,
                                                           _torch_stream(signal)))
     else:
@@ -413,6 +420,9 @@ def _r2c_with_planner(sfx, dtype, x, out_re, out_im, planner):
             raise PhastFTPanic(6)
         if ni != half + 1:
             raise PhastFTPanic(7)
+        if not _pair_aligned(x):                                  # the input is read as pairs: an aligned copy
+            x = x.clone()
+            px = C.c_void_p(x.data_ptr())
         check(fn("phastft_r2c_{s}_dev", sfx)(planner._h, px, pr, pi, _torch_stream(x)))
     else:
         px, nx = _np_ptr(x, dtype, False)
@@ -423,6 +433,7 @@ def _r2c_with_planner(sfx, dtype, x, out_re, out_im, planner):
 
 def _c2r_with_planner(sfx, dtype, in_re, in_im, out, planner, scratch_re=None, scratch_im=None):
     if _is_torch(out):
+        import torch
         pr, nr = _torch_ptr(in_re, dtype)
         pi, ni = _torch_ptr(in_im, dtype)
         po, no = _torch_ptr(out, dtype)
@@ -441,7 +452,10 @@ def _c2r_with_planner(sfx, dtype, in_re, in_im, out, planner, scratch_re=None, s
                 raise PhastFTPanic(11)
             if nsi != half:
                 raise PhastFTPanic(12)
-        check(fn("phastft_c2r_{s}_dev", sfx)(planner._h, pr, pi, po, psr, psi, _torch_stream(out)))
+        work = out if _pair_aligned(out) else torch.empty_like(out)    # the output is written as pairs: an aligned temporary
+        check(fn("phastft_c2r_{s}_dev", sfx)(planner._h, pr, pi, C.c_void_p(work.data_ptr()), psr, psi, _torch_stream(out)))
+        if work is not out:
+            out.copy_(work)
     else:
         pr, nr = _np_ptr(in_re, dtype, False)
         pi, ni = _np_ptr(in_im, dtype, False)

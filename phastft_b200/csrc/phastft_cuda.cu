@@ -42,6 +42,32 @@ int32_t fail(int32_t code, const std::string& detail = std::string()) {
     return code;
 }
 
+// The kernels the calling thread's most recent execution call launched (phastft_last_launches): one record per launch,
+// appended where the launch is made and cleared at the start of every public execution entry point.
+struct LaunchRec {
+    const char* kind;    // COL / TRANS / ROW, CLUSTER, PIPE, or an elementwise r2c / c2r kernel
+    int R, R2, C, NT, variant;   // R2: second pass size of the one-launch pairs (CLUSTER, PIPE), else 0
+    const char* mode;    // plain / tma / bulk / row-bulk / c2r-in / cluster / pipe
+    bool pdl;            // launched with programmatic dependent launch (PHASTFT_PDL=1)
+};
+thread_local std::vector<LaunchRec> g_launch_log;
+thread_local std::string g_launch_text;
+
+void launches_reset() { g_launch_log.clear(); }
+void note_launch(const LaunchRec& r) {
+    g_launch_log.push_back(r);
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+}
+const char* mode_name(int mode) {
+    switch (mode) {
+        case MODE_TMA_IN: return "tma";
+        case MODE_BULK_IN: return "bulk";
+        case MODE_ROW_BULK: return "row-bulk";
+        case MODE_C2R_IN: return "c2r-in";
+        default: return "plain";
+    }
+}
+
 #define CUDA_TRY(expr)                                                                                  \
     do {                                                                                                \
         cudaError_t _e = (expr);                                                                        \
@@ -180,6 +206,14 @@ inline uint64_t fnv1a(const std::string& str) {
 }
 constexpr int ALT_ROW_PASS = -1;   // launch_pass(): use Plan::alt_row
 
+// A batch is processed in chunks so the workspace stays bounded.  Keeping a chunk's intermediate L2-resident was
+// measured SLOWER than few large launches (4096 x 2^16 f32: L2-sized chunks, larger chunks and no chunking, fastest
+// last), so the default chunk is as large as the workspace cap allows (PHASTFT_L2_CHUNK_MB overrides).
+constexpr size_t L2_CHUNK_BYTES_DEFAULT = size_t(4) << 30;
+// The pipelined launch's ring (PHASTFT_PIPE_RING_MB): 16 MiB is about a third of the H100's 50 MB L2, so the ring can stay
+// resident beside the input and output streaming through (not measured).
+constexpr long PIPE_RING_MB_DEFAULT = 16;
+
 template <typename T>
 struct PassDesc {
     const KernelEntry<T>* k = nullptr;    // kernel for a lone transform
@@ -242,6 +276,11 @@ struct Plan {
     mutable cudaEvent_t ws_free = nullptr;   // orders workspace reuse across streams
     mutable cudaStream_t ws_last_stream = nullptr;
     mutable bool ws_used = false;
+    // launch knobs, read when the plan is built like every other PHASTFT_* setting
+    bool pdl = false;                   // PHASTFT_PDL=1: programmatic dependent launch of the passes
+    size_t l2_chunk_bytes = 0;          // PHASTFT_L2_CHUNK_MB: signal bytes per chunk of a batched multi-pass call
+    size_t pipe_ring_bytes = 0;         // PHASTFT_PIPE_RING_MB: workspace ring of the pipelined launch
+    bool pipe_discard = true;           // PHASTFT_PIPE_DISCARD=0 keeps the ring's lines in L2 after pass 2 reads them
     std::string description;
 
     ~Plan() {
@@ -461,6 +500,15 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
     std::vector<int> f = ln == 0 ? std::vector<int>{} : choose_factors<T>(ln);
     pl->num_passes = (int)f.size();
     pl->ws_il = ws_interleaved_mode();
+    if (const char* e = getenv("PHASTFT_PDL")) pl->pdl = atoi(e) != 0;
+    pl->l2_chunk_bytes = L2_CHUNK_BYTES_DEFAULT;
+    if (const char* e = getenv("PHASTFT_L2_CHUNK_MB")) { const long mb = atol(e); if (mb > 0) pl->l2_chunk_bytes = (size_t)mb << 20; }
+    {
+        long mb = PIPE_RING_MB_DEFAULT;
+        if (const char* e = getenv("PHASTFT_PIPE_RING_MB")) mb = atol(e);
+        pl->pipe_ring_bytes = (size_t)std::max(1L, mb) << 20;
+    }
+    if (const char* e = getenv("PHASTFT_PIPE_DISCARD")) pl->pipe_discard = atoi(e) != 0;
     const bool il3 = pl->num_passes == 3 && pl->ws_il != 0;   // the middle pass reads and writes interleaved data
     // two-level W_N table
     pl->lo_bits = (ln + 1) / 2;
@@ -811,8 +859,9 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
             }
         }
         if (pl->num_passes >= 2) s += pl->ws_il == 1 ? " [interleaved intermediates]" : pl->ws_il == 0 ? " [planar intermediates]" : "";
-        if (pl->pipe_b) s += std::string(" [batches: one pipelined launch, ") + (pl->pipe_b->mode ? "TMA / bulk tile input, " : "") + std::to_string(pl->pipe_grid_b) + " resident CTAs, L2 ring]";
-        if (pl->pipe_1) s += " [lone: one pipelined launch, " + std::to_string(pl->pipe_grid_1) + " resident CTAs]";
+        const std::string ring = "L2 ring of " + std::to_string(pl->pipe_ring_bytes >> 20) + " MiB";
+        if (pl->pipe_b) s += std::string(" [batches: one pipelined launch, ") + (pl->pipe_b->mode ? "TMA / bulk tile input, " : "") + std::to_string(pl->pipe_grid_b) + " resident CTAs, " + ring + "]";
+        if (pl->pipe_1) s += " [lone: one pipelined launch, " + std::to_string(pl->pipe_grid_1) + " resident CTAs, " + ring + "]";
         if (pl->alt_row.k) s += " || batches: ROW R=" + std::to_string(pl->alt_row.k->R) + "(" + pl->alt_row.k->radices + ")";
         if ((pl->num_passes == 1 && pl->pass[0].kr) || pl->alt_row.kr) s += " [contiguous planar batches: tile in / out by cp.async.bulk]";
         if (pl->cl)
@@ -885,10 +934,8 @@ int32_t launch_pass(const Plan<T>& pl, int p, const PassParams<T>& base, size_t 
     }
     void* args[] = {&prm};
     // Programmatic dependent launch: measured no gain with 128 KB tiles (the next grid cannot become resident early), -10%
-    // at 2^24+, and slower too with the 64 KB asynchronous-input tiles.  PHASTFT_PDL=1 enables it.
-    static const int pdl_env = [] { const char* e = getenv("PHASTFT_PDL"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
-    const bool use_pdl = pdl_env > 0;     // off by default: measured slower with and without the asynchronous-input kernels
-    if (use_pdl) {
+    // at 2^24+, and slower too with the 64 KB asynchronous-input tiles.  PHASTFT_PDL=1 enables it (Plan::pdl).
+    if (pl.pdl) {                          // off by default: measured slower with and without the asynchronous-input kernels
         // Programmatic dependent launch: back-to-back passes overlap the next grid's launch and prologue
         // with the previous grid's tail (the kernel waits with griddepcontrol.wait before its first access).
         prm.pdl = 1;
@@ -903,7 +950,7 @@ int32_t launch_pass(const Plan<T>& pl, int p, const PassParams<T>& base, size_t 
     } else {
         CUDA_TRY(cudaLaunchKernel(k->fn, dim3((unsigned)blocks), dim3(k->NT), args, k->smem, stream));
     }
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    note_launch({kind_name(k->kind), k->R, 0, k->C, k->NT, k->variant, mode_name(k->mode), pl.pdl});
     return PHASTFT_OK;
 }
 
@@ -967,34 +1014,13 @@ int32_t prepare_pass_desc(const Plan<T>& pl, const PassDesc<T>& d, int p, const 
     return PHASTFT_OK;
 }
 
-// A batch is processed in chunks so the workspace stays bounded.  Keeping a chunk's intermediate L2-resident was
-// measured SLOWER than few large launches (4096 x 2^16 f32: L2-sized chunks, larger chunks and no chunking, fastest
-// last), so the default chunk is as large as the workspace cap allows (PHASTFT_L2_CHUNK_MB overrides).
-constexpr size_t L2_CHUNK_BYTES_DEFAULT = size_t(4) << 30;
-inline size_t l2_chunk_bytes() {
-    static const size_t v = [] {
-        if (const char* env = getenv("PHASTFT_L2_CHUNK_MB")) { long mb = atol(env); if (mb > 0) return (size_t)mb << 20; }
-        return L2_CHUNK_BYTES_DEFAULT;
-    }();
-    return v;
-}
-
 // Ring of workspace slots of the pipelined two-pass launch: the largest power-of-two number of transforms whose
-// intermediates fit PHASTFT_PIPE_RING_MB (default 16 MiB: about a third of the H100's 50 MB L2, so the ring can stay resident
-// beside the input and output streaming through; not measured), at least 1.
-inline size_t pipe_ring_bytes() {
-    static const size_t v = [] {
-        long mb = 16;
-        if (const char* env = getenv("PHASTFT_PIPE_RING_MB")) mb = atol(env);
-        return (size_t)std::max(1L, mb) << 20;
-    }();
-    return v;
-}
+// intermediates fit Plan::pipe_ring_bytes, at least 1.
 template <typename T>
 size_t pipe_ring_transforms(const Plan<T>& pl, size_t batch) {
     const size_t bytes_per = pl.n * 2 * sizeof(T);
     size_t ring = 1;
-    while (ring * 2 * bytes_per <= pipe_ring_bytes() && ring * 2 <= batch) ring *= 2;
+    while (ring * 2 * bytes_per <= pl.pipe_ring_bytes && ring * 2 <= batch) ring *= 2;
     if (ring < 2 && batch > 1) ring = 2;            // two slots at least: pass 1 of b+1 beside pass 2 of b
     return ring;
 }
@@ -1019,7 +1045,7 @@ int32_t plan_reserve(const Plan<T>* pl, size_t batch) {
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> lock(pl->mu);
     const size_t bytes_per = pl->n * 2 * sizeof(T);
-    size_t chunk = std::max<size_t>(1, l2_chunk_bytes() / bytes_per);
+    size_t chunk = std::max<size_t>(1, pl->l2_chunk_bytes / bytes_per);
     chunk = std::min(chunk, batch);
     if (pl->pipe_b && (batch << pl->log2n) >= (size_t(1) << 21)) chunk = pipe_ring_transforms(*pl, batch);
     return grow_workspace(*pl, chunk, nullptr);
@@ -1097,7 +1123,7 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
             cfg.attrs = attr; cfg.numAttrs = 1;
             if (pass_events && done == 0) CUDA_TRY(cudaEventRecord(pass_events[0], stream));
             CUDA_TRY(cudaLaunchKernelExC(&cfg, pl.cl->fn, args));
-            g_launches.fetch_add(1, std::memory_order_relaxed);
+            note_launch({"CLUSTER", pl.cl->k1.R, pl.cl->k2.R, pl.cl->K, pl.cl->NT, pl.cl->variant, "cluster", false});
             if (pass_events && done == 0)
                 for (int q = 1; q <= pl.num_passes; ++q) CUDA_TRY(cudaEventRecord(pass_events[q], stream));
         }
@@ -1106,7 +1132,7 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
     // multi-pass: in -> ws (COL) [-> ws (COL)] -> out (TRANS), batch processed in L2-sized chunks
     std::lock_guard<std::mutex> lock(pl.mu);
     const size_t bytes_per = pl.n * 2 * sizeof(T);
-    size_t chunk = std::max<size_t>(1, l2_chunk_bytes() / bytes_per);
+    size_t chunk = std::max<size_t>(1, pl.l2_chunk_bytes / bytes_per);
     chunk = std::min(chunk, batch);
     if (pl.num_passes == 3 && pl.ws2_re != nullptr) chunk = 1;
     // pipelined two-pass launch (see fft_pipe2_kernel): the workspace is a ring of transforms instead of the whole chunk
@@ -1182,15 +1208,14 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
         ctl.tiles1 = (unsigned)(t1 / batch); ctl.tiles2 = (unsigned)(t2 / batch);
         ctl.batch = (unsigned)batch; ctl.ring = (unsigned)ring;
         ctl.delay = lone ? 1u : (unsigned)std::max<size_t>(1, ring / 2);
-        static const int discard_env = [] { const char* e = getenv("PHASTFT_PIPE_DISCARD"); return e ? atoi(e) : 1; }();
-        ctl.discard = (discard_env && il_p == 1 && !lone) ? 1 : 0;
+        ctl.discard = (pl.pipe_discard && il_p == 1 && !lone) ? 1 : 0;
         CUDA_TRY(cudaMemsetAsync(pl.pipe_state, 0, 64 + 2 * pl.pipe_state_batch * sizeof(unsigned), stream));
         const unsigned long long items = (unsigned long long)(batch + ctl.delay) * (ctl.tiles1 + ctl.tiles2);
         if (items > 0x7fffffffULL) return fail(PHASTFT_ERR_INVALID_ARG, "grid too large");
         const unsigned grid = (unsigned)items;                               // one CTA per work item (a ticket decides which)
         void* args[] = {&p1, &p2, &ctl};
         CUDA_TRY(cudaLaunchKernel(pipe->fn, dim3(grid), dim3(pipe->NT), args, pipe->smem, stream));
-        g_launches.fetch_add(1, std::memory_order_relaxed);
+        note_launch({"PIPE", pipe->R1, pipe->R2, pipe->C1, pipe->NT, 0, pipe->mode ? "pipe-tma" : "pipe", false});
         if (!capturing) {
             CUDA_TRY(cudaEventRecord(pl.ws_free, stream));
             pl.ws_last_stream = stream;
@@ -1298,6 +1323,16 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
     return PHASTFT_OK;
 }
 
+// The kernels move interleaved data as (re, im) pairs: one 2 * sizeof(T)-byte access per complex value.  A pointer the
+// device entry points read or write that way must be aligned to it (the host-slice entry points stage through aligned
+// plan buffers).
+template <typename T>
+int32_t check_pair_alignment(const T* p, const char* what) {
+    if (reinterpret_cast<uintptr_t>(p) % (2 * sizeof(T)) == 0) return PHASTFT_OK;
+    return fail(PHASTFT_ERR_INVALID_ARG, std::string(what) + " must be aligned to " + std::to_string(2 * sizeof(T)) +
+                                             " bytes (it is accessed as interleaved (re, im) pairs)");
+}
+
 template <typename T>
 int32_t check_c2c_args(const Plan<T>* pl, size_t len_re, size_t len_im, int direction) {
     if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
@@ -1351,6 +1386,7 @@ int32_t fft_interleaved_dev(const Plan<T>* pl, T* d_sig, int direction, size_t b
     if (!pl || !d_sig) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
     if (direction != PHASTFT_FORWARD && direction != PHASTFT_REVERSE) return fail(PHASTFT_ERR_INVALID_ARG, "direction must be 1 or -1");
     if (batch > 1 && bstride < pl->n) return fail(PHASTFT_ERR_INVALID_ARG, "batch_stride < N");
+    if (int32_t st = check_pair_alignment(d_sig, "d_signal")) return st;
     DeviceGuard g(pl->device);
     if (pl->num_passes == 0) return PHASTFT_OK;
     Io<T> io;
@@ -1808,6 +1844,7 @@ Tw2 r2c_tw2(const PlanR2c<T>* pl) {
 template <typename T>
 int32_t r2c_dev(const PlanR2c<T>* pl, const T* d_in, T* d_ore, T* d_oim, cudaStream_t stream) {
     if (!pl || !d_in || !d_ore || !d_oim) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
+    if (int32_t st = check_pair_alignment(d_in, "d_input")) return st;     // read as (x[2k], x[2k+1]) pairs
     DeviceGuard g(pl->device);
     const size_t half = pl->n / 2;
     // (1)+(2) deinterleave fused into the first pass load: z[k] = x[2k] + i x[2k+1] (r2c.rs:557-569),
@@ -1827,7 +1864,7 @@ int32_t r2c_dev(const PlanR2c<T>* pl, const T* d_in, T* d_ore, T* d_oim, cudaStr
     dim3 grid((unsigned)((q + 1 + 255) / 256), 1);
     r2c_untangle_kernel<T><<<grid, 256, 0, stream>>>(rp);
     CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    note_launch({"R2C-UNTANGLE", (int)half, 0, 1, 256, 0, "plain", false});
     return PHASTFT_OK;
 }
 
@@ -1835,6 +1872,7 @@ template <typename T>
 int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, T* d_sre, T* d_sim, cudaStream_t stream) {
     if (!pl || !d_ire || !d_iim || !d_out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
     if ((d_sre == nullptr) != (d_sim == nullptr)) return fail(PHASTFT_ERR_INVALID_ARG, "pass both scratch arrays or neither");
+    if (int32_t st = check_pair_alignment(d_out, "d_output")) return st;   // written as (y[2k], y[2k+1]) pairs, fused or not
     DeviceGuard g(pl->device);
     const size_t half = pl->n / 2;
     // Pre-processing (r2c.rs:764-780) folded into the loads of the inverse transform's first pass when the plan has that
@@ -1873,7 +1911,7 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
     dim3 grid((unsigned)((half + 255) / 256), 1);
     c2r_preprocess_kernel<T><<<grid, 256, 0, stream>>>(rp);
     CUDA_TRY(cudaGetLastError());
-    g_launches.fetch_add(1, std::memory_order_relaxed);
+    note_launch({"C2R-PRE", (int)half, 0, 1, 256, 0, "plain", false});
     // (2) inverse half-length c2c on the scratch (swap trick + 1/half, r2c.rs:782) with
     // (3) the re-interleave into the real output (r2c.rs:790-798) fused into the last store
     Io<T> io;
@@ -1998,6 +2036,18 @@ void phastft_oneshot_cache_clear(void) {
 }
 
 uint64_t phastft_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+const char* phastft_last_launches(void) {
+    std::string& s = g_launch_text;
+    s.clear();
+    for (const LaunchRec& r : g_launch_log) {
+        if (!s.empty()) s += "; ";
+        s += std::string(r.kind) + " R=" + std::to_string(r.R);
+        if (r.R2) s += "x" + std::to_string(r.R2);
+        s += (strcmp(r.kind, "CLUSTER") == 0 ? " K=" : " C=") + std::to_string(r.C) + " NT=" + std::to_string(r.NT) + " v" +
+             std::to_string(r.variant) + " " + r.mode + (r.pdl ? " pdl" : "");
+    }
+    return s.c_str();
+}
 int32_t phastft_device_count(int* count) {
     if (!count) return fail(PHASTFT_ERR_INVALID_ARG, "count == NULL");
     *count = 0;
@@ -2075,28 +2125,35 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     int32_t phastft_fft_dit_##SFX##_host(const phastft_plan_dit_##SFX* p, T* re, size_t lre, T* im, size_t lim,        \
                                          int dir, const phastft_options* opts) {                                        \
         (void)opts;                                                                                                     \
+        launches_reset();                                                                                               \
         return fft_host<T>(AS_CPLAN(T, p), re, lre, im, lim, dir);                                                      \
     }                                                                                                                   \
     int32_t phastft_fft_dit_##SFX##_oneshot(T* re, size_t lre, T* im, size_t lim, int dir, int device) {                \
+        launches_reset();                                                                                               \
         return fft_oneshot<T>(re, lre, im, lim, dir, device);                                                           \
     }                                                                                                                   \
     int32_t phastft_fft_dit_##SFX##_dev(const phastft_plan_dit_##SFX* p, T* re, T* im, int dir, size_t batch,          \
                                         size_t bstride, void* s) {                                                      \
+        launches_reset();                                                                                               \
         return fft_dev<T>(AS_CPLAN(T, p), re, im, dir, batch, bstride, (cudaStream_t)s);                                \
     }                                                                                                                   \
     int32_t phastft_fft_dit_##SFX##_dev_profile(const phastft_plan_dit_##SFX* p, T* re, T* im, int dir, size_t batch,  \
                                                 size_t bstride, void* s, float* pass_ms, int* num_passes) {             \
+        launches_reset();                                                                                               \
         return fft_dev_profile<T>(AS_CPLAN(T, p), re, im, dir, batch, bstride, (cudaStream_t)s, pass_ms, num_passes);   \
     }                                                                                                                   \
     int32_t phastft_fft_dit_##SFX##_batch_sharded_host(phastft_plan_dit_##SFX* const* plans, int np, T* re, T* im,     \
                                                        size_t batch, size_t bstride, int dir) {                         \
+        launches_reset();                                                                                               \
         return batch_sharded_host<T>(reinterpret_cast<Plan<T>* const*>(plans), np, re, im, batch, bstride, dir);        \
     }                                                                                                                   \
     int32_t phastft_fft_interleaved_##SFX##_host(const phastft_plan_dit_##SFX* p, T* sig, size_t len, int dir) {        \
+        launches_reset();                                                                                               \
         return fft_interleaved_host<T>(AS_CPLAN(T, p), sig, len, dir);                                                  \
     }                                                                                                                   \
     int32_t phastft_fft_interleaved_##SFX##_dev(const phastft_plan_dit_##SFX* p, T* sig, int dir, size_t batch,        \
                                                 size_t bstride, void* s) {                                              \
+        launches_reset();                                                                                               \
         return fft_interleaved_dev<T>(AS_CPLAN(T, p), sig, dir, batch, bstride, (cudaStream_t)s);                       \
     }                                                                                                                   \
     int32_t phastft_plan_r2c_##SFX##_create(size_t n, int device, phastft_plan_r2c_##SFX** out) {                       \
@@ -2110,9 +2167,11 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     size_t phastft_plan_r2c_##SFX##_size(const phastft_plan_r2c_##SFX* p) { return p ? AS_CR2C(T, p)->n : 0; }          \
     int32_t phastft_r2c_##SFX##_host(const phastft_plan_r2c_##SFX* p, const T* in, size_t lin, T* ore, size_t lore,    \
                                      T* oim, size_t loim) {                                                             \
+        launches_reset();                                                                                               \
         return r2c_host<T>(AS_CR2C(T, p), in, lin, ore, lore, oim, loim);                                               \
     }                                                                                                                   \
     int32_t phastft_r2c_##SFX##_oneshot(const T* in, size_t lin, T* ore, size_t lore, T* oim, size_t loim, int dev) {   \
+        launches_reset();                                                                                               \
         PlanR2c<T>* pl = nullptr; /* r2c.rs:522: PlannerR2c::new(input_re.len()), kept for the next same-size call */  \
         auto& c = oneshot_r2c_cache<T>();                                                                               \
         std::lock_guard<std::mutex> lock(c.mu);                                                                         \
@@ -2121,14 +2180,17 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
         return r2c_host<T>(pl, in, lin, ore, lore, oim, loim);                                                          \
     }                                                                                                                   \
     int32_t phastft_r2c_##SFX##_dev(const phastft_plan_r2c_##SFX* p, const T* in, T* ore, T* oim, void* s) {            \
+        launches_reset();                                                                                               \
         return r2c_dev<T>(AS_CR2C(T, p), in, ore, oim, (cudaStream_t)s);                                                \
     }                                                                                                                   \
     int32_t phastft_c2r_##SFX##_host(const phastft_plan_r2c_##SFX* p, const T* ire, size_t lire, const T* iim,          \
                                      size_t liim, T* out, size_t lout, T* sre, size_t lsre, T* sim, size_t lsim) {      \
+        launches_reset();                                                                                               \
         return c2r_host<T>(AS_CR2C(T, p), ire, lire, iim, liim, out, lout, sre, lsre, sim, lsim);                       \
     }                                                                                                                   \
     int32_t phastft_c2r_##SFX##_oneshot(const T* ire, size_t lire, const T* iim, size_t liim, T* out, size_t lout,     \
                                         int dev) {                                                                      \
+        launches_reset();                                                                                               \
         PlanR2c<T>* pl = nullptr; /* r2c.rs:696: PlannerR2c::new(output.len()), kept for the next same-size call */    \
         auto& c = oneshot_r2c_cache<T>();                                                                               \
         std::lock_guard<std::mutex> lock(c.mu);                                                                         \
@@ -2138,6 +2200,7 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     }                                                                                                                   \
     int32_t phastft_c2r_##SFX##_dev(const phastft_plan_r2c_##SFX* p, const T* ire, const T* iim, T* out, T* sre,        \
                                     T* sim, void* s) {                                                                  \
+        launches_reset();                                                                                               \
         return c2r_dev<T>(AS_CR2C(T, p), ire, iim, out, sre, sim, (cudaStream_t)s);                                     \
     }
 

@@ -138,6 +138,19 @@ def test_tune_candidates_host_logic(pf):
         _lib.plan_tune_candidates(12, 64)
 
 
+def test_launch_knobs_are_read_per_plan():
+    """Every PHASTFT_* knob is read when a plan is built: a getenv behind a function-local static would freeze the first value
+    the process saw, so a later plan (or a test that sets the knob) could not change it."""
+    src = (ROOT / "phastft_b200" / "csrc" / "phastft_cuda.cu").read_text()
+    for m in re.finditer(r"\bstatic\b[^;{]*=\s*\[[^\]]*\]\s*(\([^)]*\))?\s*\{", src):
+        depth, i = 1, m.end()
+        while depth:
+            depth += {"{": 1, "}": -1}.get(src[i], 0)
+            i += 1
+        assert "getenv" not in src[m.start():i], src[m.start():i]
+    assert "getenv" in src
+
+
 def test_rust_ffi_is_generated_from_the_header():
     """rust/src/ffi.rs binds every PHASTFT_API declaration: it is the output of tools/gen_rust_ffi.py on the current header."""
     import importlib.util

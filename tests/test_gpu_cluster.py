@@ -260,6 +260,7 @@ def test_pipelined_launch_is_bit_identical_to_two_launches(dt, log_n, batch, rin
     n = 1 << log_n
     rng = np.random.default_rng(log_n * 1000 + batch)
     re_h = rng.uniform(-1, 1, batch * n).astype(dt); im_h = rng.uniform(-1, 1, batch * n).astype(dt)
+    monkeypatch.setenv("PHASTFT_ONE_CTA_MAX", "13")        # else f32 2^14 batches take the one-CTA kernel, not the two passes
     monkeypatch.setenv("PHASTFT_PIPE", "0")
     plain = planner_cls(dt)(n, 0)
     assert "pipelined" not in plain.describe()
@@ -270,6 +271,7 @@ def test_pipelined_launch_is_bit_identical_to_two_launches(dt, log_n, batch, rin
     monkeypatch.setenv("PHASTFT_PIPE_TMA", str(tma))        # the 2^16 pairs also exist with TMA / bulk tile input; other sizes fall back
     piped = planner_cls(dt)(n, 0)
     assert "one pipelined launch" in piped.describe(), piped.describe()
+    assert f"L2 ring of {ring_mb} MiB" in piped.describe(), piped.describe()     # the ring size is read per plan
     if tma and log_n == 16:
         assert "TMA / bulk tile input" in piped.describe(), piped.describe()
     elif tma:
@@ -280,6 +282,7 @@ def test_pipelined_launch_is_bit_identical_to_two_launches(dt, log_n, batch, rin
     before = pf.launch_count()
     pf.fft_dit_batch(b_re, b_im, pf.Direction.Forward, piped, batch)
     assert pf.launch_count() - before == 1
+    assert [r.split()[0] for r in pf.last_launches()] == ["PIPE"], pf.last_launches()
     assert torch.equal(a_re, b_re) and torch.equal(a_im, b_im)
     # and the inverse brings the input back
     pf.fft_dit_batch(b_re, b_im, pf.Direction.Reverse, piped, batch)
