@@ -176,6 +176,15 @@ PHASTFT_API void phastft_plan_r2c_f64_destroy(phastft_plan_r2c_f64* plan);
 PHASTFT_API void phastft_plan_r2c_f32_destroy(phastft_plan_r2c_f32* plan);
 PHASTFT_API size_t phastft_plan_r2c_f64_size(const phastft_plan_r2c_f64* plan);
 PHASTFT_API size_t phastft_plan_r2c_f32_size(const phastft_plan_r2c_f32* plan);
+/* The path c2r calls on this plan take under the current environment, then the first pass's c2r build and the inner
+ * N/2-point plan's own description, e.g.
+ *   "n=2^20 f64 r2c/c2r: c2r fused on load (the first pass loads the half-spectrum) | c2r-in build: COL R=512 C=8 NT=256 R1=32
+ *    | inner: n=2^19 f64: ..."
+ * "fused on load" (the first pass builds its input from the half-spectrum; launch record mode c2r-in) or "separate sweep"
+ * (a C2R-PRE launch into scratch first), with the rule that decided in parentheses.  The string is rebuilt per call and stays
+ * valid until the calling thread's next call of either describe function. */
+PHASTFT_API const char* phastft_plan_r2c_f64_describe(const phastft_plan_r2c_f64* plan);
+PHASTFT_API const char* phastft_plan_r2c_f32_describe(const phastft_plan_r2c_f32* plan);
 
 /* ---- algorithms/r2c.rs:521-662 : r2c_fft_{f64,f32}[_with_planner] --------------------------
  * input (length N, not modified) -> output_re/output_im (length N/2+1 each).  Length checks in

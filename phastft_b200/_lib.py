@@ -95,6 +95,7 @@ SIGNATURES = {
     "phastft_plan_r2c_{s}_create": ([_sz, _ci, C.POINTER(_vp)], _i32),
     "phastft_plan_r2c_{s}_destroy": ([_vp], None),
     "phastft_plan_r2c_{s}_size": ([_vp], _sz),
+    "phastft_plan_r2c_{s}_describe": ([_vp], C.c_char_p),
     "phastft_r2c_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
     "phastft_r2c_{s}_oneshot": ([_vp, _sz, _vp, _sz, _vp, _sz, _ci], _i32),
     "phastft_r2c_{s}_dev": ([_vp, _vp, _vp, _vp, _vp], _i32),

@@ -193,6 +193,11 @@ class _PlannerR2c:
     def new(cls, n: int, device: int = 0):
         return cls(n, device)
 
+    def describe(self) -> str:
+        """The c2r path under the current environment (fused on load or the separate sweep, and why), the first pass's
+        c2r build, and the inner N/2-point plan's describe()."""
+        return fn("phastft_plan_r2c_{s}_describe", self._sfx)(self._h).decode()
+
     def __del__(self):
         h = getattr(self, "_h", None)
         if h:

@@ -52,6 +52,7 @@ struct LaunchRec {
 };
 thread_local std::vector<LaunchRec> g_launch_log;
 thread_local std::string g_launch_text;
+thread_local std::string g_r2c_desc_text;   // phastft_plan_r2c_*_describe: built per call (it reads the environment)
 
 void launches_reset() { g_launch_log.clear(); }
 void note_launch(const LaunchRec& r) {
@@ -1868,6 +1869,46 @@ int32_t r2c_dev(const PlanR2c<T>* pl, const T* d_in, T* d_ore, T* d_oim, cudaStr
     return PHASTFT_OK;
 }
 
+// Whether c2r_dev folds the pre-processing (r2c.rs:764-780) into the loads of the inverse transform's first pass under the
+// current environment, and why (`why`: the rule that decided).  Fused: no scratch, one HBM round trip of N/2 complex values
+// less.  PHASTFT_C2R_FUSE=0 keeps the separate sweep.
+template <typename T>
+bool c2r_fuses(const PlanR2c<T>* pl, const char** why) {
+    const char* fuse_e = getenv("PHASTFT_C2R_FUSE");
+    const Plan<T>& in = *pl->inner;
+    const char* r = "the first pass loads the half-spectrum";
+    bool fuse = false;
+    if (fuse_e && atoi(fuse_e) == 0) r = "PHASTFT_C2R_FUSE=0";
+    else if (in.num_passes < 2) r = "one-CTA inner plan";
+    else if (!in.pass[0].kc) r = "the first pass tile has no c2r build";
+    else if (in.cl && in.cl_min_batch <= 1) r = "lone transforms take the cluster launch";
+    else if (in.pipe_1) r = "lone transforms take the pipelined launch";
+    // Measured faster for f64 up to N = 2^20 and from 2^24 and for every f32 size; f64 2^21..2^23 (the sweep's scratch round
+    // trip is cheap there, and the 1024-row tile of 2^21 keeps only 8 of its 32 loads per thread in flight) measured slightly
+    // slower: those keep the separate sweep unless PHASTFT_C2R_FUSE=1 is set.
+    else if (!(sizeof(T) == 4 || in.log2n < 20 || in.log2n > 22 || fuse_e != nullptr))
+        r = "f64 inner 2^20..2^22 measured faster with the sweep (PHASTFT_C2R_FUSE=1 fuses)";
+    else fuse = true;
+    if (why) *why = r;
+    return fuse;
+}
+
+template <typename T>
+std::string r2c_description(const PlanR2c<T>* pl) {
+    const char* why = nullptr;
+    const bool fuse = c2r_fuses(pl, &why);
+    const Plan<T>& in = *pl->inner;
+    std::string s = "n=2^" + std::to_string(ilog2(pl->n)) + (sizeof(T) == 8 ? " f64" : " f32") + " r2c/c2r: c2r " +
+                    (fuse ? "fused on load" : "separate sweep") + " (" + why + ") | c2r-in build: ";
+    const KernelEntry<T>* kc = in.num_passes >= 2 ? in.pass[0].kc : nullptr;
+    if (kc)
+        s += std::string(kind_name(kc->kind)) + " R=" + std::to_string(kc->R) + " C=" + std::to_string(kc->C) + " NT=" +
+             std::to_string(kc->NT) + " R1=" + std::to_string(kc->first_radix);
+    else
+        s += "none";
+    return s + " | inner: " + in.description;
+}
+
 template <typename T>
 int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, T* d_sre, T* d_sim, cudaStream_t stream) {
     if (!pl || !d_ire || !d_iim || !d_out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
@@ -1875,16 +1916,8 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
     if (int32_t st = check_pair_alignment(d_out, "d_output")) return st;   // written as (y[2k], y[2k+1]) pairs, fused or not
     DeviceGuard g(pl->device);
     const size_t half = pl->n / 2;
-    // Pre-processing (r2c.rs:764-780) folded into the loads of the inverse transform's first pass when the plan has that
-    // kernel: no scratch, one HBM round trip of N/2 complex values less.  PHASTFT_C2R_FUSE=0 keeps the separate sweep.
-    const char* fuse_e = getenv("PHASTFT_C2R_FUSE");
-    const bool fuse_env = fuse_e ? atoi(fuse_e) != 0 : true;
     const Plan<T>& in = *pl->inner;
-    // Measured faster for f64 up to N = 2^20 and from 2^24 and for every f32 size; f64 2^21..2^23 (the sweep's scratch round
-    // trip is cheap there, and the 1024-row tile of 2^21 keeps only 8 of its 32 loads per thread in flight) measured slightly
-    // slower: those keep the separate sweep unless PHASTFT_C2R_FUSE=1 is set.
-    const bool fuse_size = sizeof(T) == 4 || in.log2n < 20 || in.log2n > 22 || fuse_e != nullptr;
-    if (fuse_env && fuse_size && in.num_passes >= 2 && in.pass[0].kc && !(in.cl && in.cl_min_batch <= 1) && !in.pipe_1) {
+    if (c2r_fuses(pl, nullptr)) {
         Io<T> io;
         io.in_re = d_ire; io.in_im = d_iim; io.in_il = 0; io.in_bstride = (long long)half;
         io.pre_tw2 = r2c_tw2(pl); io.pre_log2half = ilog2(half); io.pre_wc = pl->pre_wc;
@@ -2165,6 +2198,11 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     }                                                                                                                   \
     void phastft_plan_r2c_##SFX##_destroy(phastft_plan_r2c_##SFX* p) { delete AS_R2C(T, p); }                           \
     size_t phastft_plan_r2c_##SFX##_size(const phastft_plan_r2c_##SFX* p) { return p ? AS_CR2C(T, p)->n : 0; }          \
+    const char* phastft_plan_r2c_##SFX##_describe(const phastft_plan_r2c_##SFX* p) {                                    \
+        if (!p) return "";                                                                                              \
+        g_r2c_desc_text = r2c_description<T>(AS_CR2C(T, p));                                                            \
+        return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
     int32_t phastft_r2c_##SFX##_host(const phastft_plan_r2c_##SFX* p, const T* in, size_t lin, T* ore, size_t lore,    \
                                      T* oim, size_t loim) {                                                             \
         launches_reset();                                                                                               \

@@ -28,7 +28,8 @@ def test_header_declares_expected_surface():
     syms = declared_symbols()
     assert len(syms) >= 50
     for must in ("phastft_fft_dit_f64_host", "phastft_fft_dit_f32_dev", "phastft_r2c_f64_dev", "phastft_c2r_f32_host",
-                 "phastft_plan_dit_f64_tables_broadcast", "phastft_fft_dit_f32_batch_sharded_host"):
+                 "phastft_plan_dit_f64_tables_broadcast", "phastft_fft_dit_f32_batch_sharded_host", "phastft_plan_r2c_f64_describe",
+                 "phastft_plan_r2c_f32_describe"):
         assert must in syms
 
 

@@ -193,3 +193,161 @@ def test_mutations_fail_the_device_checks(log_n):
     Y[1], Y[n - 1] = Y[n - 1], Y[1]
     with pytest.raises(AssertionError):
         T.impulse_check(torch.from_numpy(Y.real.copy()), torch.from_numpy(Y.imag.copy()), pos, a_re, a_im, n, False, np.float64, "swapped")
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# real transforms: the r2c / c2r device checks, the long-double model of the reference's c2r, and their mutation tests
+# ------------------------------------------------------------------------------------------------------------------------
+def _t(a):
+    import torch
+    return torch.from_numpy(np.ascontiguousarray(a, np.float64))
+
+
+@pytest.mark.parametrize("log_n", [12, 14, 16])
+def test_real_device_checks_agree_with_long_double(log_n):
+    import torch
+    n, half = 1 << log_n, 1 << (log_n - 1)
+    f = [(log_n - 1) // 2, log_n - 1 - (log_n - 1) // 2]
+    # r2c: sampled bins (0, N/4, N/2, pairs k / N/2 - k) against rfft_ld; the rounded long-double spectrum passes every check
+    R = T.r2c_truth(log_n, n)
+    bins = T.half_bins(n, f)
+    assert {0, n // 4, half} <= set(bins) and all(half - k in bins for k in bins) and len(bins) >= 64
+    w_re, w_im = T.r2c_sampled_bins(log_n, n, bins)
+    d = np.abs((w_re.numpy() + 1j * w_im.numpy()).astype(np.clongdouble) - R[bins])
+    assert float(d.max()) / np.sqrt(T.real_signal_energy(log_n, n)) <= T.C_REF_SAMPLED * E64 * np.sqrt(log_n)
+    X_re, X_im = _t(R.real), _t(R.imag)
+    T.r2c_sampled_check(X_re, X_im, log_n, n, bins, np.float64, "rfft_ld")
+    T.half_parseval_check(X_re, X_im, T.real_signal_energy(log_n, n), n, np.float64, "rfft_ld")
+    pos = T.impulse_positions(n, [1] + f)
+    amp = T.impulse_amplitudes(len(pos))[0]
+    x = np.zeros(n)
+    x[pos] = amp
+    Y = T.rfft_ld(x)
+    T.impulse_check(_t(Y.real), _t(Y.imag), pos, amp, np.zeros(len(pos)), n, False, np.float64, "rfft_ld impulses", count=half + 1)
+    s_re, s_im = T.real_impulse_spectrum(pos, amp, n)
+    assert float(np.max(np.abs((s_re.numpy() + 1j * s_im.numpy()) - Y))) <= T.C_REF_IMPULSE * E64 * np.sqrt(log_n) * float(np.max(np.abs(Y)))
+    # c2r: sampled outputs of hermitian_spectrum and its energy against irfft_ld; impulses back from their closed-form spectrum
+    y = T.c2r_truth(log_n, n)
+    ts = T.c2r_positions(n, f)
+    assert {half - 1, half, n - 1, 0, 1} <= set(ts) and all(t ^ 1 in ts for t in ts)
+    want = T.c2r_sampled_outputs(log_n, n, ts).numpy()
+    rms = np.sqrt(T.hermitian_energy(log_n, n) / n)
+    assert abs(rms / float(np.sqrt(np.mean(y.astype(np.float64) ** 2))) - 1) < 1e-12
+    assert float(np.max(np.abs(want.astype(np.longdouble) - y[ts]))) / rms <= T.C_REF_SAMPLED * E64 * np.sqrt(log_n)
+    T.c2r_sampled_check(_t(y), log_n, n, ts, np.float64, "irfft_ld")
+    back = T.irfft_ld(s_re.numpy(), s_im.numpy(), n)
+    T.c2r_impulse_check(_t(back), pos, amp, n, np.float64, "irfft_ld impulses")
+    T.c2r_impulse_check(torch.from_numpy(back.astype(np.float32)), pos, amp, n, np.float32, "irfft_ld impulses, f32")
+
+
+@pytest.mark.parametrize("log_n", [2, 3, 4, 8, 12, 16])
+def test_c2r_model(log_n):
+    """The long-double model of the reference's c2r: irfft on valid spectra, and not irfft where the DC or Nyquist bin has an
+    imaginary part."""
+    n = 1 << log_n
+    h_re, h_im = T.hermitian_spectrum(log_n, n)
+    m = T.c2r_model_ld(h_re, h_im, n)
+    want = T.c2r_truth(log_n, n)
+    assert float(np.max(np.abs(m - want))) <= 1e-2 * E64 * float(np.max(np.abs(want)))
+    s_re, s_im = T.c2r_spectrum(log_n, n)
+    assert s_im[0] != 0 and s_im[-1] != 0
+    g = T.c2r_model_truth(log_n, n)
+    assert float(np.max(np.abs(g - T.irfft_ld(s_re, s_im, n)))) > 1e6 * E64 * float(np.max(np.abs(g)))
+
+
+@pytest.mark.parametrize("dt", [np.float64, np.float32])
+@pytest.mark.parametrize("log_n", [2, 3, 6, 10, 14])
+def test_c2r_model_matches_the_oracle(dt, log_n):
+    """On non-Hermitian input the oracle (the reference restated) meets the model within its own error on valid input."""
+    import sys
+    sys.path.insert(0, str(GOLD.parent.parent))
+    from oracle import oracle as O
+    O.build()
+    n = 1 << log_n
+    errs = []
+    for spec, want in ((T.hermitian_spectrum(log_n, n), T.c2r_truth(log_n, n)), (T.c2r_spectrum(log_n, n), T.c2r_model_truth(log_n, n))):
+        y = np.zeros(n, dt)
+        O.c2r_fft(spec[0].astype(dt), spec[1].astype(dt), y)
+        errs.append(T.errors(y, None, want))
+    (l_h, r_h), (l_n, r_n) = errs
+    e = T.eps(dt)
+    assert l_n <= max(2 * l_h, T.bound_linf(dt, n)) and r_n <= max(2 * r_h, T.bound_rms(dt, n)), (l_h / e, r_h / e, l_n / e, r_n / e)
+
+
+def _r2c_mutants(X, want, n, k):
+    """k: a sampled bin other than 0, N/4, N/2 (a wrong kernel would swap whole families of bins; the checks see one pair)."""
+    half = n // 2
+    out = {"conjugated": np.conj(X)}
+    sw = X.copy()
+    sw[k], sw[half - k] = X[half - k], X[k]
+    out["bins k and N/2 - k swapped"] = sw
+    q = X.copy()
+    q[n // 4] += 8 * E64 * float(np.max(np.abs(want))) * np.exp(0.3j)
+    out["error at N/4 only"] = q
+    ny = X.copy()
+    ny[half] = -ny[half]
+    out["wrong Nyquist bin"] = ny
+    out["error x10"] = (want + 10 * (X.astype(np.clongdouble) - want)).astype(np.complex128)
+    return out
+
+
+@pytest.mark.parametrize("log_n", [12, 16])
+def test_r2c_mutations_fail(log_n):
+    n, half = 1 << log_n, 1 << (log_n - 1)
+    f = [(log_n - 1) // 2, log_n - 1 - (log_n - 1) // 2]
+    x = T.signal(log_n, n, real=True)
+    want = T.r2c_truth(log_n, n)
+    X = np.fft.rfft(x)
+    T.check(X.real, X.imag, want, np.float64, n, "pocketfft rfft")
+    bins = T.half_bins(n, f)
+    T.r2c_sampled_check(_t(X.real), _t(X.imag), log_n, n, bins, np.float64, "pocketfft rfft")
+    T.half_parseval_check(_t(X.real), _t(X.imag), T.real_signal_energy(log_n, n), n, np.float64, "pocketfft rfft")
+    k = next(b for b in bins[len(bins) // 3:] if b not in (n // 4, half))
+    for name, M in _r2c_mutants(X, want, n, k).items():
+        linf, rms = T.errors(M.real, M.imag, want)
+        assert linf > T.bound_linf(np.float64, n) or rms > T.bound_rms(np.float64, n), name
+        if name == "error x10":
+            assert linf <= T.old_bound(np.float64, n)
+            continue
+        with pytest.raises(AssertionError):
+            T.r2c_sampled_check(_t(M.real), _t(M.imag), log_n, n, bins, np.float64, name)
+    # real impulses: a swapped pair of bins fails the closed form
+    pos = T.impulse_positions(n, [1] + f)
+    amp = T.impulse_amplitudes(len(pos))[0]
+    z = np.zeros(n)
+    z[pos] = amp
+    Y = np.fft.rfft(z)
+    T.impulse_check(_t(Y.real), _t(Y.imag), pos, amp, np.zeros(len(pos)), n, False, np.float64, "pocketfft", count=half + 1)
+    Y[3], Y[half - 3] = Y[half - 3], Y[3]
+    with pytest.raises(AssertionError):
+        T.impulse_check(_t(Y.real), _t(Y.imag), pos, amp, np.zeros(len(pos)), n, False, np.float64, "swapped", count=half + 1)
+
+
+@pytest.mark.parametrize("log_n", [12, 16])
+def test_c2r_mutations_fail(log_n):
+    n = 1 << log_n
+    f = [(log_n - 1) // 2, log_n - 1 - (log_n - 1) // 2]
+    h_re, h_im = T.hermitian_spectrum(log_n, n)
+    want = T.c2r_truth(log_n, n)
+    y = np.fft.irfft(h_re + 1j * h_im, n)
+    T.check(y, None, want, np.float64, n, "pocketfft irfft")
+    ts = T.c2r_positions(n, f)
+    T.c2r_sampled_check(_t(y), log_n, n, ts, np.float64, "pocketfft irfft")
+    pos = T.impulse_positions(n, [1] + f)
+    amp = T.impulse_amplitudes(len(pos))[0]
+    s_re, s_im = T.real_impulse_spectrum(pos, amp, n)
+    yi = np.fft.irfft(s_re.numpy() + 1j * s_im.numpy(), n)
+    T.c2r_impulse_check(_t(yi), pos, amp, n, np.float64, "pocketfft irfft")
+    pairs = lambda v: v.reshape(-1, 2)[:, ::-1].reshape(-1).copy()            # noqa: E731
+    muts = {"pairs swapped": (pairs(y), pairs(yi)), "scaled by 2": (2 * y, 2 * yi),
+            "error x10": ((want + 10 * (y.astype(np.longdouble) - want)).astype(np.float64), None)}
+    for name, (M, Mi) in muts.items():
+        linf, rms = T.errors(M, None, want)
+        assert linf > T.bound_linf(np.float64, n) or rms > T.bound_rms(np.float64, n), name
+        if Mi is None:
+            assert linf <= T.old_bound(np.float64, n)
+            continue
+        with pytest.raises(AssertionError):
+            T.c2r_sampled_check(_t(M), log_n, n, ts, np.float64, name)
+        with pytest.raises(AssertionError):
+            T.c2r_impulse_check(_t(Mi), pos, amp, n, np.float64, name)

@@ -3,8 +3,9 @@
 * Long-double FFTs (`fft_ld`, `rfft_ld`, `irfft_ld`): NumPy's FFT computes `clongdouble` input in long double (64-bit
   mantissa on x86-64), far more accurate than any f64 or f32 result it judges.  Used up to 2^26 points.
 * Device checks (`sampled_bins`, `impulse_check`, `parseval_check`), in torch so they run on CUDA and CPU tensors alike: for sizes
-  whose long-double FFT would not fit the host (2^27..2^30).  Every phase is reduced exactly in int64, (k*n) mod N, before
-  it becomes an angle.
+  whose long-double FFT would not fit the host (2^27..2^31).  Every phase is reduced exactly in int64, (k*n) mod N, before
+  it becomes an angle.  The real transforms have their own: `r2c_sampled_check`, `half_parseval_check`, `c2r_sampled_check`,
+  `c2r_impulse_check`, and `c2r_model_ld`, the reference's c2r in long double for any half-spectrum.
 * Inputs come from a counter-based hash of the index (`signal`, `signal_torch`), so any chunk of a 2^30-point signal can
   be rebuilt without keeping a copy.  Its values are multiples of 2^-23 in [-1, 1): exact in f32 and f64, so both precisions
   transform the same signal and share one reference.
@@ -23,6 +24,7 @@ if np.finfo(np.longdouble).nmant < 63:
                       f"{np.finfo(np.longdouble).nmant}-bit mantissa)")
 
 EPS = {np.dtype(np.float64): 2.0 ** -52, np.dtype(np.float32): 2.0 ** -23}
+_PI_LD = np.longdouble("3.14159265358979323846264338327950288")
 
 # C * eps * sqrt(log2 N); set from the errors measured on an H100 (DESIGN.md section 5): at most 2x the largest
 # measured ratio per precision, and C_LINF <= 3 keeps the L-inf bound at most a quarter of 4 * eps * log2(N) from 2^10 up.
@@ -230,6 +232,38 @@ def c2r_truth(seed: int, n: int) -> np.ndarray:
     return _cached(("c2r", seed, n), lambda: irfft_ld(*hermitian_spectrum(seed, n), n))
 
 
+def c2r_model_ld(re, im, n: int) -> np.ndarray:
+    """The reference's c2r of any N/2 + 1 bins, in long double (r2c.rs:263-347, 764-798): for k < N/2
+        z[k] = (X[k] + conj(X[N/2 - k])) / 2 + i conj(W_N^k) (X[k] - conj(X[N/2 - k])) / 2,   W_N = exp(-2 pi i / N),
+    then the inverse N/2-point FFT (1/(N/2) scaled) and y[2j] = Re z'[j], y[2j + 1] = Im z'[j].  For a valid spectrum (DC and
+    Nyquist bins real) this is irfft; otherwise the imaginary parts of those two bins enter z[0], where irfft drops them."""
+    half = n // 2
+    X = np.empty(half + 1, np.clongdouble)
+    X.real = np.asarray(re, np.longdouble)
+    X.imag = np.asarray(im, np.longdouble)
+    k = np.arange(half, dtype=np.int64)
+    ang = k.astype(np.longdouble) * (2 * _PI_LD / n)       # exact: k < 2^31 and n a power of two
+    cw = np.empty(half, np.clongdouble)                      # conj(W_N^k)
+    cw.real = np.cos(ang)
+    cw.imag = np.sin(ang)
+    a, b = X[:half], np.conj(X[half - k])
+    z = (a + b) / 2 + 1j * cw * (a - b) / 2
+    zt = np.fft.ifft(z)
+    y = np.empty(n, np.longdouble)
+    y[0::2] = zt.real
+    y[1::2] = zt.imag
+    return y
+
+
+def c2r_spectrum(seed: int, n: int):
+    """N/2 + 1 hashed bins with nonzero imaginary parts at DC and Nyquist too: not the half of any real signal's spectrum."""
+    return signal(seed + 1000, n // 2 + 1)
+
+
+def c2r_model_truth(seed: int, n: int) -> np.ndarray:
+    return _cached(("c2r-model", seed, n), lambda: c2r_model_ld(*c2r_spectrum(seed, n), n))
+
+
 def clear_cache() -> None:
     _CACHE.clear()
     _SPLITS.clear()
@@ -398,9 +432,10 @@ def impulse_amplitudes(count: int, seed: int = 0):
     return a[0], a[1]
 
 
-def impulse_check(X_re, X_im, pos, a_re, a_im, n: int, inverse: bool, dt, what: str = "") -> tuple:
+def impulse_check(X_re, X_im, pos, a_re, a_im, n: int, inverse: bool, dt, what: str = "", count: int = None) -> tuple:
     """Every bin of the transform of sum_j a_j delta(n - n_j) against sum_j a_j W_N^(+-k n_j mod N), in f64 chunks.
-    Both metrics of `check`, with the f64 reference's own allowance.  Returns (L-inf, RMS) in eps(dt)."""
+    Both metrics of `check`, with the f64 reference's own allowance.  Returns (L-inf, RMS) in eps(dt).
+    count: check bins 0 .. count - 1 only (r2c: N/2 + 1)."""
     import torch
     dev = X_re.device
     p = torch.as_tensor(pos, dtype=torch.int64, device=dev)
@@ -408,8 +443,9 @@ def impulse_check(X_re, X_im, pos, a_re, a_im, n: int, inverse: bool, dt, what: 
     ai = torch.as_tensor(a_im, dtype=torch.float64, device=dev)[:, None]
     num_max = den_max = num_sq = den_sq = 0.0
     step = max(1, (1 << 26) // len(pos))
-    for s in range(0, n, step):
-        m = min(step, n - s)
+    count = n if count is None else count
+    for s in range(0, count, step):
+        m = min(step, count - s)
         k = torch.arange(s, s + m, dtype=torch.int64, device=dev)
         c, sn = _phase(k, p, n, inverse)        # [J, m]: exp(-+2 pi i n_j k / N)
         w_re = (ar * c - ai * sn).sum(dim=0)
@@ -447,3 +483,189 @@ def parseval_check(X_re, X_im, energy_x: float, n: int, inverse: bool, dt, what:
     rel = abs(e_X / want - 1.0)
     assert rel <= 2 * bound_rms(dt, n) + C_REF_IMPULSE * EPS[np.dtype(np.float64)] * np.sqrt(_lg(n)), (what, n, "Parseval", rel / eps(dt))
     return rel / eps(dt)
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# device checks of the real transforms (r2c: N/2 + 1 bins of a real signal; c2r: N reals from N/2 + 1 bins)
+# ------------------------------------------------------------------------------------------------------------------------
+def half_bins(n: int, inner_log2_factors, count: int = 64, seed: int = 0) -> list:
+    """r2c bins to sample, all in [0, N/2]: 0, N/4 (the bin the untangle pairs with itself), N/2, and every bin next to a digit
+    boundary of the inner N/2-point plan (boundary_bins) together with its partner N/2 - k (the untangle computes k and
+    N/2 - k together, so a mix-up of the two shows at both)."""
+    half = n // 2
+    ks = {0, n // 4, half}
+    for k in boundary_bins(half, inner_log2_factors, count, seed):
+        ks |= {k, half - k}
+    return sorted(ks)
+
+
+def c2r_positions(n: int, inner_log2_factors, count: int = 64, seed: int = 0) -> list:
+    """c2r output samples to check: both reals (2j, 2j + 1) of every inner output j next to a digit boundary, and of the
+    inner outputs holding N/2 - 1, N/2 and N - 1."""
+    js = set(boundary_bins(n // 2, inner_log2_factors, count, seed)) | {max(n // 4 - 1, 0), n // 4, n // 2 - 1}
+    return sorted({t for j in js for t in (2 * j, 2 * j + 1)})
+
+
+def _fsum_columns(parts) -> np.ndarray:
+    import math
+    a = np.stack(parts)
+    return np.array([math.fsum(a[:, i]) for i in range(a.shape[1])])
+
+
+def r2c_sampled_bins(seed: int, n: int, bins, device="cpu"):
+    """Direct f64 sums X[k] = sum_t x[t] W_N^(k t) of signal(seed, n, real=True) at `bins`; chunk sums added exactly."""
+    import torch
+    k = torch.as_tensor(list(bins), dtype=torch.int64, device=device)
+    parts_re, parts_im = [], []
+    step = max(1, (1 << 26) // max(1, len(bins)))
+    for s in range(0, n, step):
+        m = min(step, n - s)
+        x = signal_torch(seed, m, s, device, real=True)
+        c, sn = _phase(torch.arange(s, s + m, dtype=torch.int64, device=device), k, n, False)
+        parts_re.append((c * x).sum(dim=1).cpu().numpy())
+        parts_im.append((sn * x).sum(dim=1).cpu().numpy())
+    return (torch.as_tensor(_fsum_columns(parts_re), dtype=torch.float64, device=device),
+            torch.as_tensor(_fsum_columns(parts_im), dtype=torch.float64, device=device))
+
+
+def real_signal_energy(seed: int, n: int, device="cpu") -> float:
+    import math
+    tot = []
+    step = 1 << 24
+    for s in range(0, n, step):
+        x = signal_torch(seed, min(step, n - s), s, device, real=True)
+        tot.append(float((x * x).sum()))
+    return math.fsum(tot)
+
+
+def _sampled_allow(dt, n: int) -> float:
+    r = np.sqrt(_lg(n))
+    return C_SAMPLED * eps(dt) * r + C_REF_SAMPLED * EPS[np.dtype(np.float64)] * r
+
+
+def r2c_sampled_check(X_re, X_im, seed: int, n: int, bins, dt, what: str = "") -> float:
+    """r2c bins against their direct sums, relative to rms|X*| (= ||x||, Parseval over all N bins), under the bound of
+    sampled_check.  Returns the error in eps(dt)."""
+    import torch
+    dev = X_re.device
+    w_re, w_im = r2c_sampled_bins(seed, n, bins, dev)
+    k = torch.as_tensor(list(bins), dtype=torch.int64, device=dev)
+    err = float(torch.sqrt((X_re[k].to(torch.float64) - w_re) ** 2 + (X_im[k].to(torch.float64) - w_im) ** 2).max())
+    rel = err / np.sqrt(real_signal_energy(seed, n, dev))
+    r = np.sqrt(_lg(n))
+    print(f"[accuracy] {what} {np.dtype(dt).name} 2^{int(np.log2(n))}: r2c sampled bins {rel / eps(dt):.2f} eps of rms|X| "
+          f"({rel / eps(dt) / r:.3f} sqrt(lgN))")
+    assert rel <= _sampled_allow(dt, n), (what, n, np.dtype(dt).name, "r2c sampled bins", rel / eps(dt), _sampled_allow(dt, n) / eps(dt))
+    return rel / eps(dt)
+
+
+def half_parseval_check(X_re, X_im, energy_x: float, n: int, dt, what: str = "") -> float:
+    """sum_k w_k |X_k|^2 over the N/2 + 1 bins, w = 1, 2, ..., 2, 1, equals N sum x^2; held to parseval_check's bound."""
+    import torch
+    half = n // 2
+    e_X = 0.0
+    step = 1 << 24
+    for s in range(0, half + 1, step):
+        a = X_re[s:s + step].to(torch.float64)
+        b = X_im[s:s + step].to(torch.float64)
+        e_X += 2.0 * float((a * a + b * b).sum())
+    for k in (0, half):
+        e_X -= float(X_re[k]) ** 2 + float(X_im[k]) ** 2
+    rel = abs(e_X / (energy_x * n) - 1.0)
+    allow = 2 * bound_rms(dt, n) + C_REF_IMPULSE * EPS[np.dtype(np.float64)] * np.sqrt(_lg(n))
+    assert rel <= allow, (what, n, "half-spectrum Parseval", rel / eps(dt), allow / eps(dt))
+    return rel / eps(dt)
+
+
+def c2r_sampled_outputs(seed: int, n: int, ts, device="cpu"):
+    """Direct f64 sums of the c2r of hermitian_spectrum(seed, n) at samples `ts`:
+    y[t] = (1/N) sum_{k=0}^{N/2} w_k (Re X_k cos(2 pi k t / N) - Im X_k sin(2 pi k t / N)),  w = 1, 2, ..., 2, 1
+    (the imaginary parts of the DC and Nyquist bins are zero).  The spectrum is rebuilt in chunks where the tensors live."""
+    import torch
+    half = n // 2
+    t = torch.as_tensor(list(ts), dtype=torch.int64, device=device)
+    parts = []
+    step = max(1, (1 << 26) // max(1, len(ts)))
+    for s in range(0, half + 1, step):
+        m = min(step, half + 1 - s)
+        a, b = signal_torch(seed, m, s, device)
+        k = torch.arange(s, s + m, dtype=torch.int64, device=device)
+        w = torch.where((k == 0) | (k == half), 1.0, 2.0).to(torch.float64)
+        b = torch.where((k == 0) | (k == half), 0.0, b)
+        c, sn = _phase(k, t, n, True)              # [T, m]: exp(+2 pi i t k / N)
+        parts.append((c * (w * a) - sn * (w * b)).sum(dim=1).cpu().numpy())
+    return torch.as_tensor(_fsum_columns(parts) / n, dtype=torch.float64, device=device)
+
+
+def hermitian_energy(seed: int, n: int, device="cpu") -> float:
+    """sum_t y[t]^2 of the c2r of hermitian_spectrum(seed, n): (1/N) sum_k w_k |X_k|^2 (Parseval), in chunks."""
+    import math
+    half = n // 2
+    tot = []
+    step = 1 << 24
+    for s in range(0, half + 1, step):
+        a, b = signal_torch(seed, min(step, half + 1 - s), s, device)
+        tot.append(2.0 * float((a * a + b * b).sum()))
+    re0, im0 = signal(seed, 1)
+    reh, imh = signal(seed, 1, half)
+    tot += [-(re0[0] ** 2 + 2 * im0[0] ** 2), -(reh[0] ** 2 + 2 * imh[0] ** 2)]     # w = 1 and no imaginary part at DC, Nyquist
+    return math.fsum(tot) / n
+
+
+def c2r_sampled_check(y, seed: int, n: int, ts, dt, what: str = "") -> float:
+    """c2r output samples against their direct sums, relative to rms|y*|, under the bound of sampled_check."""
+    import torch
+    dev = y.device
+    want = c2r_sampled_outputs(seed, n, ts, dev)
+    t = torch.as_tensor(list(ts), dtype=torch.int64, device=dev)
+    err = float((y[t].to(torch.float64) - want).abs().max())
+    rel = err / np.sqrt(hermitian_energy(seed, n, dev) / n)
+    r = np.sqrt(_lg(n))
+    print(f"[accuracy] {what} {np.dtype(dt).name} 2^{int(np.log2(n))}: c2r sampled outputs {rel / eps(dt):.2f} eps of rms|y| "
+          f"({rel / eps(dt) / r:.3f} sqrt(lgN))")
+    assert rel <= _sampled_allow(dt, n), (what, n, np.dtype(dt).name, "c2r sampled outputs", rel / eps(dt), _sampled_allow(dt, n) / eps(dt))
+    return rel / eps(dt)
+
+
+def real_impulse_spectrum(pos, amp, n: int, device="cpu", out=None):
+    """The closed form X_k = sum_j a_j W_N^(k p_j), k = 0..N/2, of the real impulses a_j at p_j, in f64 chunks; written into
+    `out` (two tensors of N/2 + 1 elements, rounded to their type) when given."""
+    import torch
+    half = n // 2
+    p = torch.as_tensor(list(pos), dtype=torch.int64, device=device)
+    a = torch.as_tensor(np.asarray(amp), dtype=torch.float64, device=device)[:, None]
+    if out is None:
+        out = (torch.empty(half + 1, dtype=torch.float64, device=device), torch.empty(half + 1, dtype=torch.float64, device=device))
+    out_re, out_im = out
+    step = max(1, (1 << 26) // len(pos))
+    for s in range(0, half + 1, step):
+        m = min(step, half + 1 - s)
+        c, sn = _phase(torch.arange(s, s + m, dtype=torch.int64, device=device), p, n, False)
+        out_re[s:s + m] = (a * c).sum(dim=0)
+        out_im[s:s + m] = (a * sn).sum(dim=0)
+    return out_re, out_im
+
+
+def c2r_impulse_check(y, pos, amp, n: int, dt, what: str = "") -> tuple:
+    """c2r of real_impulse_spectrum(pos, amp, n), rounded to dt, must return the impulses at every sample.  Allowed on top of
+    the bounds of `check`: the f64 closed form's own error (as impulse_check) and the spectrum's rounding to dt, which moves
+    the exact result by at most eps(dt)/2 in relative RMS (Parseval); the same is allowed on L-inf."""
+    import torch
+    a = np.asarray(amp, np.float64)
+    num_max = num_sq = 0.0
+    step = 1 << 24
+    for s in range(0, n, step):
+        d = y[s:s + step].to(torch.float64).abs()
+        for p, v in zip(pos, a):
+            if s <= p < s + step:
+                d[p - s] = abs(float(y[p]) - v)
+        num_max = max(num_max, float(d.max()))
+        num_sq += float((d * d).sum())
+    linf, rms = num_max / float(np.abs(a).max()), float(np.sqrt(num_sq / float(np.dot(a, a))))
+    e, r = eps(dt), np.sqrt(_lg(n))
+    ref = C_REF_IMPULSE * EPS[np.dtype(np.float64)] * r + 0.5 * (eps(dt) if np.dtype(dt) != np.float64 else 0.0)
+    print(f"[accuracy] {what} {np.dtype(dt).name} 2^{int(np.log2(n))}: c2r impulses L-inf {linf / e:.2f} eps ({linf / e / r:.3f} sqrt(lgN)), "
+          f"RMS {rms / e:.2f} eps ({rms / e / r:.3f} sqrt(lgN))")
+    assert linf <= bound_linf(dt, n) + ref, (what, n, np.dtype(dt).name, "c2r impulses L-inf", linf / e)
+    assert rms <= bound_rms(dt, n) + ref, (what, n, np.dtype(dt).name, "c2r impulses RMS", rms / e)
+    return linf / e, rms / e
