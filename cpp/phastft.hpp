@@ -62,6 +62,10 @@ template <> struct Api<double> {
     static int32_t c2r_oneshot(const double* ire, std::size_t lre, const double* iim, std::size_t lim, double* out, std::size_t lo) { return phastft_c2r_f64_oneshot(ire, lre, iim, lim, out, lo, 0); }
     static int32_t fft_host(const Dit* p, double* re, std::size_t lr, double* im, std::size_t li, int d) { return phastft_fft_dit_f64_host(p, re, lr, im, li, d, nullptr); }
     static int32_t r2c_create(std::size_t n, int dev, R2c** o) { return phastft_plan_r2c_f64_create(n, dev, o); }
+    static int32_t r2c_reserve(const R2c* p, std::size_t b) { return phastft_plan_r2c_f64_reserve(p, b); }
+    static const char* r2c_describe(const R2c* p, std::size_t b) { return phastft_plan_r2c_f64_describe_batch(p, b); }
+    static int32_t r2c_batch_dev(const R2c* p, const double* in, std::size_t is, double* ore, double* oim, std::size_t os, std::size_t b, void* s) { return phastft_r2c_f64_batch_dev(p, in, is, ore, oim, os, b, s); }
+    static int32_t c2r_batch_dev(const R2c* p, const double* ire, const double* iim, std::size_t is, double* out, std::size_t os, double* sre, double* sim, std::size_t b, void* s) { return phastft_c2r_f64_batch_dev(p, ire, iim, is, out, os, sre, sim, b, s); }
     static void r2c_destroy(R2c* p) { phastft_plan_r2c_f64_destroy(p); }
     static int32_t r2c_host(const R2c* p, const double* in, std::size_t li, double* ore, std::size_t lre, double* oim, std::size_t lim) { return phastft_r2c_f64_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const double* ire, std::size_t lre, const double* iim, std::size_t lim, double* out, std::size_t lo, double* sre, std::size_t lsr, double* sim, std::size_t lsi) { return phastft_c2r_f64_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
@@ -79,6 +83,10 @@ template <> struct Api<float> {
     static int32_t c2r_oneshot(const float* ire, std::size_t lre, const float* iim, std::size_t lim, float* out, std::size_t lo) { return phastft_c2r_f32_oneshot(ire, lre, iim, lim, out, lo, 0); }
     static int32_t fft_host(const Dit* p, float* re, std::size_t lr, float* im, std::size_t li, int d) { return phastft_fft_dit_f32_host(p, re, lr, im, li, d, nullptr); }
     static int32_t r2c_create(std::size_t n, int dev, R2c** o) { return phastft_plan_r2c_f32_create(n, dev, o); }
+    static int32_t r2c_reserve(const R2c* p, std::size_t b) { return phastft_plan_r2c_f32_reserve(p, b); }
+    static const char* r2c_describe(const R2c* p, std::size_t b) { return phastft_plan_r2c_f32_describe_batch(p, b); }
+    static int32_t r2c_batch_dev(const R2c* p, const float* in, std::size_t is, float* ore, float* oim, std::size_t os, std::size_t b, void* s) { return phastft_r2c_f32_batch_dev(p, in, is, ore, oim, os, b, s); }
+    static int32_t c2r_batch_dev(const R2c* p, const float* ire, const float* iim, std::size_t is, float* out, std::size_t os, float* sre, float* sim, std::size_t b, void* s) { return phastft_c2r_f32_batch_dev(p, ire, iim, is, out, os, sre, sim, b, s); }
     static void r2c_destroy(R2c* p) { phastft_plan_r2c_f32_destroy(p); }
     static int32_t r2c_host(const R2c* p, const float* in, std::size_t li, float* ore, std::size_t lre, float* oim, std::size_t lim) { return phastft_r2c_f32_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const float* ire, std::size_t lre, const float* iim, std::size_t lim, float* out, std::size_t lo, float* sre, std::size_t lsr, float* sim, std::size_t lsi) { return phastft_c2r_f32_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
@@ -116,6 +124,20 @@ class PlannerR2c {
     PlannerR2c(const PlannerR2c&) = delete;
     PlannerR2c& operator=(const PlannerR2c&) = delete;
     const typename Api<T>::R2c* raw() const { return raw_; }
+    /// additive: the c2r path calls of `batch` transforms take (describe_batch; batch 1 = describe)
+    std::string describe(std::size_t batch = 1) const { return Api<T>::r2c_describe(raw_, batch); }
+    /// additive: make every allocation a batched call of `batch` transforms would make now
+    void reserve(std::size_t batch) const { check(Api<T>::r2c_reserve(raw_, batch)); }
+    /// additive: `batch` r2c transforms on device pointers, member b at b * in_stride reals / b * out_stride bins
+    void r2c_batch_dev(const T* d_in, std::size_t in_stride, T* d_out_re, T* d_out_im, std::size_t out_stride, std::size_t batch,
+                       void* stream = nullptr) const {
+        check(Api<T>::r2c_batch_dev(raw_, d_in, in_stride, d_out_re, d_out_im, out_stride, batch, stream));
+    }
+    /// additive: `batch` c2r transforms; scratch batch * N/2 each, dense, or both null for the plan's own
+    void c2r_batch_dev(const T* d_in_re, const T* d_in_im, std::size_t in_stride, T* d_out, std::size_t out_stride, std::size_t batch,
+                       T* d_scratch_re = nullptr, T* d_scratch_im = nullptr, void* stream = nullptr) const {
+        check(Api<T>::c2r_batch_dev(raw_, d_in_re, d_in_im, in_stride, d_out, out_stride, d_scratch_re, d_scratch_im, batch, stream));
+    }
   private:
     typename Api<T>::R2c* raw_ = nullptr;
 };

@@ -185,6 +185,16 @@ PHASTFT_API size_t phastft_plan_r2c_f32_size(const phastft_plan_r2c_f32* plan);
  * valid until the calling thread's next call of either describe function. */
 PHASTFT_API const char* phastft_plan_r2c_f64_describe(const phastft_plan_r2c_f64* plan);
 PHASTFT_API const char* phastft_plan_r2c_f32_describe(const phastft_plan_r2c_f32* plan);
+/* The same for batched calls of `batch` transforms (phastft_{r2c,c2r}_*_batch_dev): the c2r path that batch takes, the rule that
+ * decided, and the c2r build of the first pass such a call runs ("none" where it runs a kernel without one: the one-CTA
+ * kernel, the cluster or pipelined launch, the TMA pair).  describe_batch(plan, 1) equals describe(plan). */
+PHASTFT_API const char* phastft_plan_r2c_f64_describe_batch(const phastft_plan_r2c_f64* plan, size_t batch);
+PHASTFT_API const char* phastft_plan_r2c_f32_describe_batch(const phastft_plan_r2c_f32* plan, size_t batch);
+/* Makes, now and on this thread, every allocation a batched call of `batch` transforms would make: the inner plan's workspace
+ * and, when that batch's c2r takes the separate sweep, the plan-owned c2r scratch (batch * N/2 per array).  A batched call that
+ * would grow either while its stream is being captured into a CUDA graph returns PHASTFT_ERR_INVALID_ARG instead. */
+PHASTFT_API int32_t phastft_plan_r2c_f64_reserve(const phastft_plan_r2c_f64* plan, size_t batch);
+PHASTFT_API int32_t phastft_plan_r2c_f32_reserve(const phastft_plan_r2c_f32* plan, size_t batch);
 
 /* ---- algorithms/r2c.rs:521-662 : r2c_fft_{f64,f32}[_with_planner] --------------------------
  * input (length N, not modified) -> output_re/output_im (length N/2+1 each).  Length checks in
@@ -228,6 +238,30 @@ PHASTFT_API int32_t phastft_c2r_f64_dev(const phastft_plan_r2c_f64* plan, const 
                                         double* d_output, double* d_scratch_re, double* d_scratch_im, void* stream);
 PHASTFT_API int32_t phastft_c2r_f32_dev(const phastft_plan_r2c_f32* plan, const float* d_in_re, const float* d_in_im,
                                         float* d_output, float* d_scratch_re, float* d_scratch_im, void* stream);
+
+/* ---- batched r2c / c2r, device-resident (the reference has no batch API: a batch is a caller loop) --------------------
+ * `batch` transforms in one call, asynchronous on `stream`; each member means exactly what the lone *_dev call means.
+ * Strides are in elements of the array they describe: member b of a real array starts at b * stride reals, member b of a
+ * spectrum array at b * stride bins.
+ *   r2c: in_stride >= N and even, out_stride >= N/2 + 1; writes N/2 + 1 bins per member, never writes d_input.
+ *   c2r: in_stride >= N/2 + 1, out_stride >= N and even; normalised so that c2r(r2c(x)) == x, never writes the spectra.
+ *        d_scratch_re / d_scratch_im: batch * N/2 elements each, dense, or both NULL for the plan-owned scratch (grown to
+ *        batch * N/2 on first use, or ahead of time by phastft_plan_r2c_*_reserve).
+ * The real arrays are accessed as (re, im) pairs: their base must be aligned to 2 * sizeof(T) bytes, which is why the real
+ * stride must be even.  A stride that is too small or odd, a misaligned base, one scratch pointer without the other or a
+ * NULL pointer returns PHASTFT_ERR_INVALID_ARG (the detail names the argument) before anything is launched.  batch == 0
+ * launches nothing; batch == 1 runs exactly the lone *_dev call.  The c2r path of a batch (fused into the first pass's loads
+ * or the separate sweep) is stated by phastft_plan_r2c_*_describe_batch. */
+PHASTFT_API int32_t phastft_r2c_f64_batch_dev(const phastft_plan_r2c_f64* plan, const double* d_input, size_t in_stride,
+                                              double* d_out_re, double* d_out_im, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_r2c_f32_batch_dev(const phastft_plan_r2c_f32* plan, const float* d_input, size_t in_stride,
+                                              float* d_out_re, float* d_out_im, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_c2r_f64_batch_dev(const phastft_plan_r2c_f64* plan, const double* d_in_re, const double* d_in_im,
+                                              size_t in_stride, double* d_output, size_t out_stride, double* d_scratch_re,
+                                              double* d_scratch_im, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_c2r_f32_batch_dev(const phastft_plan_r2c_f32* plan, const float* d_in_re, const float* d_in_im,
+                                              size_t in_stride, float* d_output, size_t out_stride, float* d_scratch_re,
+                                              float* d_scratch_im, size_t batch, void* stream);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

@@ -96,12 +96,16 @@ SIGNATURES = {
     "phastft_plan_r2c_{s}_destroy": ([_vp], None),
     "phastft_plan_r2c_{s}_size": ([_vp], _sz),
     "phastft_plan_r2c_{s}_describe": ([_vp], C.c_char_p),
+    "phastft_plan_r2c_{s}_describe_batch": ([_vp, _sz], C.c_char_p),
+    "phastft_plan_r2c_{s}_reserve": ([_vp, _sz], _i32),
     "phastft_r2c_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
     "phastft_r2c_{s}_oneshot": ([_vp, _sz, _vp, _sz, _vp, _sz, _ci], _i32),
     "phastft_r2c_{s}_dev": ([_vp, _vp, _vp, _vp, _vp], _i32),
     "phastft_c2r_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
     "phastft_c2r_{s}_oneshot": ([_vp, _sz, _vp, _sz, _vp, _sz, _ci], _i32),
     "phastft_c2r_{s}_dev": ([_vp, _vp, _vp, _vp, _vp, _vp, _vp], _i32),
+    "phastft_r2c_{s}_batch_dev": ([_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp], _i32),
+    "phastft_c2r_{s}_batch_dev": ([_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp], _i32),
 }
 def check(code: int):
     if code != OK:

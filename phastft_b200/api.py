@@ -38,6 +38,7 @@ __all__ = [
     "r2c_fft_f32", "r2c_fft_f32_with_planner", "c2r_fft_f32", "c2r_fft_f32_with_planner",
     "c2r_fft_f32_with_planner_and_scratch",
     "fft_dit_batch", "fft_dit_batch_sharded", "host_register", "host_unregister",
+    "r2c_batch", "c2r_batch",
 ]
 
 
@@ -193,10 +194,18 @@ class _PlannerR2c:
     def new(cls, n: int, device: int = 0):
         return cls(n, device)
 
-    def describe(self) -> str:
-        """The c2r path under the current environment (fused on load or the separate sweep, and why), the first pass's
-        c2r build, and the inner N/2-point plan's describe()."""
-        return fn("phastft_plan_r2c_{s}_describe", self._sfx)(self._h).decode()
+    def describe(self, batch: int = 1) -> str:
+        """The c2r path calls of `batch` transforms take under the current environment (fused on load or the separate
+        sweep, and why), the c2r build of the first pass they run, and the inner N/2-point plan's describe()."""
+        if batch == 1:
+            return fn("phastft_plan_r2c_{s}_describe", self._sfx)(self._h).decode()
+        return fn("phastft_plan_r2c_{s}_describe_batch", self._sfx)(self._h, int(batch)).decode()
+
+    def reserve(self, batch: int) -> None:
+        """Make every allocation a batched call of `batch` transforms would make now: the inner plan's workspace and, when
+        that batch's c2r takes the separate sweep, the plan-owned scratch (otherwise the first such call makes them,
+        synchronising the device -- an error inside a CUDA-graph capture)."""
+        check(fn("phastft_plan_r2c_{s}_reserve", self._sfx)(self._h, int(batch)))
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -553,3 +562,60 @@ def c2r_fft_f32_with_planner(input_re, input_im, output, planner: PlannerR2c32) 
 def c2r_fft_f32_with_planner_and_scratch(input_re, input_im, output, planner: PlannerR2c32, scratch_re, scratch_im) -> None:
     """r2c.rs:835"""
     _c2r_with_planner("f32", np.float32, input_re, input_im, output, planner, scratch_re, scratch_im)
+
+
+# ----------------------------------------------------------------------------------------------
+# batched r2c / c2r (device-resident; the reference has no batch API)
+# ----------------------------------------------------------------------------------------------
+def _check_batch_len(what: str, have: int, batch: int, stride: int, length: int) -> None:
+    if batch < 0:
+        raise PhastFTPanic(13, "batch < 0")
+    if batch and have < (batch - 1) * stride + length:
+        raise PhastFTPanic(13, f"{what} shorter than (batch - 1) * stride + {length}")
+
+
+def r2c_batch(x, out_re, out_im, planner, batch: int, in_stride: int | None = None, out_stride: int | None = None) -> None:
+    """`batch` r2c transforms in one call on flat 1-D torch CUDA tensors: member b reads N reals at x[b * in_stride:] and
+    writes N/2 + 1 bins at out_re / out_im[b * out_stride:] (defaults: N and N/2 + 1).  In-stride must be even (the input is
+    read as (re, im) pairs); a misaligned x is read through an aligned copy."""
+    n, half = planner.n, planner.n // 2
+    in_stride = n if in_stride is None else int(in_stride)
+    out_stride = half + 1 if out_stride is None else int(out_stride)
+    px, nx = _torch_ptr(x, planner._dtype)
+    pr, nr = _torch_ptr(out_re, planner._dtype)
+    pi, ni = _torch_ptr(out_im, planner._dtype)
+    _check_batch_len("input", nx, batch, in_stride, n)
+    _check_batch_len("output_re", nr, batch, out_stride, half + 1)
+    _check_batch_len("output_im", ni, batch, out_stride, half + 1)
+    if not _pair_aligned(x):
+        x = x.clone()
+        px = C.c_void_p(x.data_ptr())
+    check(fn("phastft_r2c_{s}_batch_dev", planner._sfx)(planner._h, px, in_stride, pr, pi, out_stride, int(batch), _torch_stream(x)))
+
+
+def c2r_batch(in_re, in_im, out, planner, batch: int, in_stride: int | None = None, out_stride: int | None = None,
+              scratch_re=None, scratch_im=None) -> None:
+    """`batch` c2r transforms in one call on flat 1-D torch CUDA tensors: member b reads N/2 + 1 bins at
+    in_re / in_im[b * in_stride:] and writes N reals at out[b * out_stride:] (defaults: N/2 + 1 and N), normalised so that
+    c2r(r2c(x)) == x.  scratch_re / scratch_im: batch * N/2 each, or neither (the planner's own).  Out-stride must be even
+    (the output is written as (re, im) pairs); a misaligned out is written through an aligned copy."""
+    n, half = planner.n, planner.n // 2
+    in_stride = half + 1 if in_stride is None else int(in_stride)
+    out_stride = n if out_stride is None else int(out_stride)
+    pr, nr = _torch_ptr(in_re, planner._dtype)
+    pi, ni = _torch_ptr(in_im, planner._dtype)
+    _, no = _torch_ptr(out, planner._dtype)
+    _check_batch_len("input_re", nr, batch, in_stride, half + 1)
+    _check_batch_len("input_im", ni, batch, in_stride, half + 1)
+    _check_batch_len("output", no, batch, out_stride, n)
+    psr = psi = None
+    if scratch_re is not None or scratch_im is not None:
+        psr, nsr = _torch_ptr(scratch_re, planner._dtype)
+        psi, nsi = _torch_ptr(scratch_im, planner._dtype)
+        if nsr < batch * half or nsi < batch * half:
+            raise PhastFTPanic(13, "scratch shorter than batch * N/2")
+    work = out if _pair_aligned(out) else out.clone()      # the clone keeps what lies between the members
+    check(fn("phastft_c2r_{s}_batch_dev", planner._sfx)(planner._h, pr, pi, in_stride, C.c_void_p(work.data_ptr()), out_stride,
+                                                        psr, psi, int(batch), _torch_stream(out)))
+    if work is not out:
+        out.copy_(work)

@@ -238,17 +238,21 @@ struct PassKernel {
     // MODE_C2R_IN: element k of the half-length inverse transform's input, built on the fly from the half-spectrum
     // (same arithmetic, in the same order, as c2r_preprocess_kernel below; r2c.rs:263-347).  The inverse runs as a forward
     // transform of the swapped parts (r2c.rs:782), so the kernel is handed (im, re).
+    // `mbase`: where the batch member's spectrum starts (member * in_bstride); a0 - mbase is the bin index.
     template <int N>
-    static __device__ __forceinline__ void gload_c2r(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N]) {
-        // element i is bin k = a0 + i * step with step = (N/2) / R1 (first pass: R * B = N/2), so its twiddle
-        // W_N^k = W_N^a0 * W_(2 R1)^i: one table lookup per task, the second factors are launch constants (pre_wc).
+    static __device__ __forceinline__ void gload_c2r(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N],
+                                                     long long mbase) {
+        // element i is bin k = k0 + i * step with step = (N/2) / R1 (first pass: R * B = N/2), so its twiddle
+        // W_N^k = W_N^k0 * W_(2 R1)^i: one table lookup per task, the second factors are launch constants (pre_wc).
+        // Its partner bin N/2 - k lies in the same member.
         // Loads in groups of 8 (f64): 4 scalars per element, all of a group in flight at once.
         const long long half = 1LL << p.pre_log2half;
+        const long long k0 = a0 - mbase;
         const T* __restrict__ fr = p.in_re + a0;
         const T* __restrict__ fi = p.in_im + a0;
-        const T* __restrict__ sr = p.in_re + (half - a0);
-        const T* __restrict__ si = p.in_im + (half - a0);
-        const double2 wb = p.pre_tw2.get((uint32_t)a0);
+        const T* __restrict__ sr = p.in_re + (mbase + half - k0);
+        const T* __restrict__ si = p.in_im + (mbase + half - k0);
+        const double2 wb = p.pre_tw2.get((uint32_t)k0);
         constexpr int G = (sizeof(T) == 8 && N > 8) ? 8 : N;
 #pragma unroll
         for (int g0 = 0; g0 < N; g0 += G) {
@@ -272,9 +276,10 @@ struct PassKernel {
         }
     }
     template <int N, int IL = -1>
-    static __device__ __forceinline__ void gload_n(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N]) {
+    static __device__ __forceinline__ void gload_n(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N],
+                                                   [[maybe_unused]] long long mbase = 0) {
         if constexpr (XCH == MODE_C2R_IN) {
-            gload_c2r<N>(p, a0, step, x);
+            gload_c2r<N>(p, a0, step, x, mbase);
         } else if constexpr (IL < 0) {
             if (p.in_interleaved == 0) gload_n<N, 0>(p, a0, step, x);
             else if (p.in_interleaved == 1) gload_n<N, 1>(p, a0, step, x);
@@ -466,6 +471,7 @@ struct PassKernel {
         uint32_t kp0 = 0;              // previous-pass output digit of column c = 0
         uint32_t kp_cstep = 0;         // ... and its increment per column
         uint32_t bcol0 = 0;            // flat index of the remaining digits for column 0 (COL only)
+        [[maybe_unused]] long long mbase = 0;   // MODE_C2R_IN: first input element of this tile's batch member
 
         if constexpr (KIND == KIND_COL) {
             const int tilesB = 1 << (p.log2B - LOG2C);
@@ -476,6 +482,7 @@ struct PassKernel {
             const int batch = rest >> p.log2A;
             const long long off = ((long long)a << (LOG2R + p.log2B)) + ((long long)bt << LOG2C);
             in_base = (long long)batch * p.in_bstride + off;
+            if constexpr (XCH == MODE_C2R_IN) mbase = (long long)batch * p.in_bstride;
             out_base = (long long)(p.out_ring ? (batch & (p.out_ring - 1)) : batch) * p.out_bstride + off;
             in_rstride = 1LL << p.log2B;
             in_cstride = 1;
@@ -570,7 +577,7 @@ struct PassKernel {
                     for (int i = 0; i < R1; ++i) pre[i] = src[i * M];
                 } else if ((KIND != KIND_ROW) || (c < rows_valid)) {
                     const long long a0 = in_base + (long long)c * in_cstride + (long long)mp * in_rstride;
-                    gload_n<R1>(p, a0, (long long)M * in_rstride, pre);
+                    gload_n<R1>(p, a0, (long long)M * in_rstride, pre, mbase);
                 } else {
 #pragma unroll
                     for (int i = 0; i < R1; ++i) pre[i] = make_cx<T>(T(0), T(0));
@@ -659,7 +666,7 @@ struct PassKernel {
                     for (int i = 0; i < R1; ++i) x[i] = pre[i];
                 } else if (valid) {
                     const long long a0 = in_base + (long long)c * in_cstride + (long long)mp * in_rstride;
-                    gload_n<R1, IL>(p, a0, (long long)M * in_rstride, x);
+                    gload_n<R1, IL>(p, a0, (long long)M * in_rstride, x, mbase);
                 } else {
 #pragma unroll
                     for (int i = 0; i < R1; ++i) x[i] = make_cx<T>(T(0), T(0));
@@ -836,6 +843,7 @@ struct RealParams {
     long long bstride;          // elements between batch members in re/im
     long long in_bstride;
     int log2half;
+    unsigned blocks_per_member; // the grid is members x blocks_per_member blocks, member-major
     Tw2 tw2;                    // two-level table for W_N, N = 2*half
 };
 
@@ -843,9 +851,10 @@ template <typename T>
 __global__ void __launch_bounds__(256) r2c_untangle_kernel(const __grid_constant__ RealParams<T> p) {
     const long long half = 1LL << p.log2half;
     const long long q = half >> 1;
-    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    T* re = p.re + (long long)blockIdx.y * p.bstride;
-    T* im = p.im + (long long)blockIdx.y * p.bstride;
+    const unsigned mb = blockIdx.x / p.blocks_per_member;
+    const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * blockDim.x + threadIdx.x;
+    T* re = p.re + (long long)mb * p.bstride;
+    T* im = p.im + (long long)mb * p.bstride;
     if (k > q) return;
     if (k == 0) {
         // r2c.rs:161-166
@@ -876,12 +885,13 @@ __global__ void __launch_bounds__(256) r2c_untangle_kernel(const __grid_constant
 template <typename T>
 __global__ void __launch_bounds__(256) c2r_preprocess_kernel(const __grid_constant__ RealParams<T> p) {
     const long long half = 1LL << p.log2half;
-    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned mb = blockIdx.x / p.blocks_per_member;
+    const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * blockDim.x + threadIdx.x;
     if (k >= half) return;
-    const T* ire = p.in_re + (long long)blockIdx.y * p.in_bstride;
-    const T* iim = p.in_im + (long long)blockIdx.y * p.in_bstride;
-    T* zre = p.re + (long long)blockIdx.y * p.bstride;
-    T* zim = p.im + (long long)blockIdx.y * p.bstride;
+    const T* ire = p.in_re + (long long)mb * p.in_bstride;
+    const T* iim = p.in_im + (long long)mb * p.in_bstride;
+    T* zre = p.re + (long long)mb * p.bstride;
+    T* zim = p.im + (long long)mb * p.bstride;
     const long long m = half - k;
     double2 wd = p.tw2.get((uint32_t)k);
     const T c_h = T(0.5 * wd.x), s_h = T(0.5 * wd.y);

@@ -221,6 +221,7 @@ struct PassDesc {
     const KernelEntry<T>* kb = nullptr;   // kernel when the call carries many transforms (multi-wave grids)
     const KernelEntry<T>* kt = nullptr;   // 2-pass plans of lone transforms: the pass with an asynchronous (TMA) tile input
     const KernelEntry<T>* kc = nullptr;   // first pass only: `k` with the c2r pre-processing folded into its loads (MODE_C2R_IN)
+    const KernelEntry<T>* kcb = nullptr;  // first pass only: the same build of `kb` (batched c2r)
     const KernelEntry<T>* kr = nullptr;   // one-CTA plans: `kb` with its tile moved in and out by cp.async.bulk (MODE_ROW_BULK)
     size_t tw_wc_off_t = (size_t)-1;      // W_L^(c*m) table for `kt`
     size_t tw_im_off = (size_t)-1;        // one-CTA kernels: the per-stage [i][m] stage-twiddle tables for `k` ...
@@ -556,8 +557,12 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
         if (kind == KIND_ROW) d.kr = find_row_bulk<T>(d.kb);
         if (p == 0 && kind == KIND_COL)         // the same tile with the c2r pre-processing in its loads, if compiled (c2r_dev uses it)
             for (const auto& e : registry<T>())
-                if (e.mode == MODE_C2R_IN && e.kind == kind && e.R == d.k->R && e.C == d.k->C && e.NT == d.k->NT &&
+                if (e.mode == MODE_C2R_IN && !e.batch_only && e.kind == kind && e.R == d.k->R && e.C == d.k->C && e.NT == d.k->NT &&
                     e.variant == d.k->variant && e.rl == d.k->rl) d.kc = &e;
+        if (p == 0 && kind == KIND_COL && d.kb)  // ... and of the batch tile (batched c2r)
+            for (const auto& e : registry<T>())
+                if (e.mode == MODE_C2R_IN && e.kind == kind && e.R == d.kb->R && e.C == d.kb->C && e.NT == d.kb->NT &&
+                    e.variant == d.kb->variant && e.rl == d.kb->rl) d.kcb = &e;
         if (p > 0) {
             d.has_tw = 1;
             d.log2Rprev = f[p - 1];
@@ -747,6 +752,8 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kt->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kt->smem));
         if (pl->pass[p].kc)
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kc->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kc->smem));
+        if (pl->pass[p].kcb)
+            CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kcb->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kcb->smem));
         if (pl->pass[p].kr)
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kr->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kr->smem));
     }
@@ -900,7 +907,14 @@ struct Io {
     Tw2 pre_tw2 = {nullptr, nullptr, 0};
     int pre_log2half = 0;
     const double2* pre_wc = nullptr;     // host: W_(2 R1)^i, i < 32 (PlanR2c::pre_wc)
+    const double2* pre_wc_b = nullptr;   // the same for the first radix of PassDesc::kcb (PlanR2c::pre_wc_b)
 };
+
+// Whether a launch of `batch` transforms of this pass runs the batch kernel PassDesc::kb (multi-wave grids).
+template <typename T>
+bool pass_takes_kb(const Plan<T>& pl, const PassDesc<T>& d, size_t batch) {
+    return d.kb != nullptr && batch > 1 && (batch << pl.log2n) >= (size_t(1) << 21);
+}
 
 // k1_lo / k1_cnt (multi-pass plans, batch == 1): restrict a pass AFTER the first to the sub-transforms
 // whose first-pass output digit k1 lies in [k1_lo, k1_lo + k1_cnt) -- the unit of L2 blocking.
@@ -971,7 +985,7 @@ template <typename T>
 int32_t prepare_pass_desc(const Plan<T>& pl, const PassDesc<T>& d, int p, const PassParams<T>& base, size_t batch, long long k1_lo,
                           long long k1_cnt, PassParams<T>& prm_out, const KernelEntry<T>*& k_out, unsigned long long& blocks_out,
                           bool use_kt) {
-    const bool many = !use_kt && d.kb != nullptr && batch > 1 && (batch << pl.log2n) >= (size_t(1) << 21);
+    const bool many = !use_kt && pass_takes_kb(pl, d, batch);
     const KernelEntry<T>* k = use_kt ? d.kt : many ? d.kb : d.k;
     // one-CTA batch kernel with bulk tile input / output: planar arrays, transforms back to back, 16-byte-aligned planes
     if (many && d.kr && k == d.kb && base.in_interleaved == 0 && base.out_interleaved == 0 && base.in_bstride == (long long)pl.n &&
@@ -980,8 +994,9 @@ int32_t prepare_pass_desc(const Plan<T>& pl, const PassDesc<T>& d, int p, const 
           reinterpret_cast<uintptr_t>(base.out_im)) & 15) == 0)
         k = d.kr;
     if (base.pre_log2half) {
-        if (p != 0 || use_kt || many || !d.kc) return fail(PHASTFT_ERR_INVALID_ARG, "c2r pre-processing on load: lone first pass with a MODE_C2R_IN kernel only");
-        k = d.kc;
+        const KernelEntry<T>* kc = many ? d.kcb : d.kc;
+        if (p != 0 || use_kt || !kc) return fail(PHASTFT_ERR_INVALID_ARG, "c2r pre-processing on load: first pass with a MODE_C2R_IN kernel only");
+        k = kc;
     }
     PassParams<T> prm = base;
     prm.batch = (int)batch;
@@ -1024,6 +1039,15 @@ size_t pipe_ring_transforms(const Plan<T>& pl, size_t batch) {
     while (ring * 2 * bytes_per <= pl.pipe_ring_bytes && ring * 2 <= batch) ring *= 2;
     if (ring < 2 && batch > 1) ring = 2;            // two slots at least: pass 1 of b+1 beside pass 2 of b
     return ring;
+}
+// Transforms per chunk of a batched multi-pass call (run_c2c).
+template <typename T>
+size_t chunk_transforms(const Plan<T>& pl, size_t batch) {
+    const size_t bytes_per = pl.n * 2 * sizeof(T);
+    size_t chunk = std::max<size_t>(1, pl.l2_chunk_bytes / bytes_per);
+    chunk = std::min(chunk, batch);
+    if (pl.num_passes == 3 && pl.ws2_re != nullptr) chunk = 1;
+    return chunk;
 }
 // caller holds pl.mu
 template <typename T>
@@ -1132,10 +1156,7 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
     }
     // multi-pass: in -> ws (COL) [-> ws (COL)] -> out (TRANS), batch processed in L2-sized chunks
     std::lock_guard<std::mutex> lock(pl.mu);
-    const size_t bytes_per = pl.n * 2 * sizeof(T);
-    size_t chunk = std::max<size_t>(1, pl.l2_chunk_bytes / bytes_per);
-    chunk = std::min(chunk, batch);
-    if (pl.num_passes == 3 && pl.ws2_re != nullptr) chunk = 1;
+    const size_t chunk = chunk_transforms(pl, batch);
     // pipelined two-pass launch (see fft_pipe2_kernel): the workspace is a ring of transforms instead of the whole chunk
     const PipeEntry<T>* pipe = nullptr;
     if (pl.num_passes == 2 && !pass_events) {
@@ -1290,7 +1311,9 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
                 prm.in_bstride = io.in_bstride;
                 prm.in_interleaved = io.in_il;
                 prm.pre_tw2 = io.pre_tw2; prm.pre_log2half = io.pre_log2half;
-                if (io.pre_wc) memcpy(prm.pre_wc, io.pre_wc, sizeof(prm.pre_wc));
+                // the W_(2 R1) factors for the first radix of the build that runs: kcb on a multi-wave chunk, else kc
+                const double2* wc = (io.pre_wc_b && pass_takes_kb(pl, pl.pass[0], nb)) ? io.pre_wc_b : io.pre_wc;
+                if (wc) memcpy(prm.pre_wc, wc, sizeof(prm.pre_wc));
             } else {
                 prm.in_re = pl.ws_re; prm.in_im = pl.ws_im; prm.in_bstride = (long long)pl.n;
                 prm.in_interleaved = il;
@@ -1781,13 +1804,15 @@ struct PlanR2c {
     size_t hi_elems = 0, lo_elems = 0;
     int lo_bits = 0;
     double2 pre_wc[32];                // W_(2 R1)^i for the fused c2r first pass (R1 = first radix of inner->pass[0].kc)
+    double2 pre_wc_b[32];              // ... and of a batched one (R1 = first radix of inner->pass[0].kcb)
     mutable std::mutex mu;
     mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then mu)
     mutable T* d_real = nullptr;       // host-API staging: N reals
     mutable T* d_spec_re = nullptr;    // N/2+1
     mutable T* d_spec_im = nullptr;
-    mutable T* d_scr_re = nullptr;     // N/2 (c2r scratch when the caller passes none)
+    mutable T* d_scr_re = nullptr;     // N/2 (c2r scratch when the caller passes none); grown under `mu` by batched sweeps
     mutable T* d_scr_im = nullptr;
+    mutable size_t scr_elems = 0;      // per array
     mutable cudaEvent_t scr_free = nullptr;        // orders reuse of the plan-owned scratch across streams (like Plan::ws_free)
     mutable cudaStream_t scr_last_stream = nullptr;
     mutable bool scr_used = false;
@@ -1821,13 +1846,19 @@ int32_t build_plan_r2c(size_t n, int device, PlanR2c<T>** out) {
     CUDA_TRY(cudaMalloc(&pl->tw_dev, tab.size() * sizeof(double2)));
     CUDA_TRY(cudaMemcpy(pl->tw_dev, tab.data(), tab.size() * sizeof(double2), cudaMemcpyHostToDevice));
     memset(pl->pre_wc, 0, sizeof(pl->pre_wc));
+    memset(pl->pre_wc_b, 0, sizeof(pl->pre_wc_b));
     if (pl->inner->num_passes >= 2 && pl->inner->pass[0].kc) {
         const uint64_t r1 = (uint64_t)pl->inner->pass[0].kc->first_radix;
         for (uint64_t i = 0; i < r1 && i < 32; ++i) root_of_unity(i, 2 * r1, pl->pre_wc[i].x, pl->pre_wc[i].y);
     }
+    if (pl->inner->num_passes >= 2 && pl->inner->pass[0].kcb) {
+        const uint64_t r1 = (uint64_t)pl->inner->pass[0].kcb->first_radix;
+        for (uint64_t i = 0; i < r1 && i < 32; ++i) root_of_unity(i, 2 * r1, pl->pre_wc_b[i].x, pl->pre_wc_b[i].y);
+    }
     // c2r scratch for the allocating variants lives in the plan (r2c.rs:716-718 allocates per call)
     CUDA_TRY(cudaMalloc(&pl->d_scr_re, (n / 2) * sizeof(T)));
     CUDA_TRY(cudaMalloc(&pl->d_scr_im, (n / 2) * sizeof(T)));
+    pl->scr_elems = n / 2;
     CUDA_TRY(cudaEventCreateWithFlags(&pl->scr_free, cudaEventDisableTiming));
     *out = pl.release();
     return PHASTFT_OK;
@@ -1840,6 +1871,28 @@ Tw2 r2c_tw2(const PlanR2c<T>* pl) {
     t.lo = t.hi + pl->hi_elems;
     t.lo_bits = pl->lo_bits;
     return t;
+}
+
+// The elementwise r2c untangle / c2r pre-processing of `members` batch members, `per` threads each: a member-major grid of
+// 256-thread blocks, so a batch is not capped by gridDim.y; a batch of more than 2^31 - 1 blocks takes several launches.
+// Launch record: R = N/2, C = the members of that launch.
+template <typename T>
+int32_t launch_real(bool untangle, const RealParams<T>& rp, size_t per, size_t members, cudaStream_t stream) {
+    const size_t bpm = (per + 255) / 256;
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    for (size_t done = 0; done < members; done += max_members) {
+        const size_t nb = std::min(members - done, max_members);
+        RealParams<T> q = rp;
+        q.re += done * rp.bstride; q.im += done * rp.bstride;
+        if (q.in_re) { q.in_re += done * rp.in_bstride; q.in_im += done * rp.in_bstride; }
+        q.blocks_per_member = (unsigned)bpm;
+        const dim3 grid((unsigned)(nb * bpm));
+        if (untangle) r2c_untangle_kernel<T><<<grid, 256, 0, stream>>>(q);
+        else c2r_preprocess_kernel<T><<<grid, 256, 0, stream>>>(q);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({untangle ? "R2C-UNTANGLE" : "C2R-PRE", 1 << rp.log2half, 0, (int)nb, 256, 0, "plain", false});
+    }
+    return PHASTFT_OK;
 }
 
 template <typename T>
@@ -1861,23 +1914,53 @@ int32_t r2c_dev(const PlanR2c<T>* pl, const T* d_in, T* d_ore, T* d_oim, cudaStr
     RealParams<T> rp;
     memset(&rp, 0, sizeof(rp));
     rp.re = d_ore; rp.im = d_oim; rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
-    const size_t q = half / 2;
-    dim3 grid((unsigned)((q + 1 + 255) / 256), 1);
-    r2c_untangle_kernel<T><<<grid, 256, 0, stream>>>(rp);
-    CUDA_TRY(cudaGetLastError());
-    note_launch({"R2C-UNTANGLE", (int)half, 0, 1, 256, 0, "plain", false});
-    return PHASTFT_OK;
+    return launch_real(true, rp, half / 2 + 1, 1, stream);
 }
 
-// Whether c2r_dev folds the pre-processing (r2c.rs:764-780) into the loads of the inverse transform's first pass under the
-// current environment, and why (`why`: the rule that decided).  Fused: no scratch, one HBM round trip of N/2 complex values
-// less.  PHASTFT_C2R_FUSE=0 keeps the separate sweep.
+// The c2r build of the first pass a batched call of `batch` > 1 transforms runs on the inner plan, or NULL when that call
+// takes a path without one (`why` says which).  The paths follow run_c2c: the one-CTA kernel, the cluster and pipelined
+// launches and the TMA pair have no c2r build; otherwise every chunk's first pass needs one (kcb on a multi-wave chunk,
+// kc on a chunk of one transform or below 2^21 points).
 template <typename T>
-bool c2r_fuses(const PlanR2c<T>* pl, const char** why) {
+const KernelEntry<T>* c2r_batch_first_pass(const Plan<T>& in, size_t batch, const char** why) {
+    const bool many_call = (batch << in.log2n) >= (size_t(1) << 21);
+    if (in.num_passes < 2) { *why = "one-CTA inner plan"; return nullptr; }
+    if (in.alt_row.k && batch >= in.alt_row_min_batch) { *why = "batches of this size take the one-CTA kernel"; return nullptr; }
+    if (in.cl && batch >= in.cl_min_batch) { *why = "batches of this size take the cluster launch"; return nullptr; }
+    if (in.num_passes == 2 && many_call && in.pipe_b) { *why = "batches of this size take the pipelined launch"; return nullptr; }
+    if (in.num_passes == 2 && in.pass[0].kt && in.pass[1].kt && many_call && in.tma_batch && in.ws_il != 0 &&
+        (batch << in.log2n) * sizeof(T) >= (size_t(32) << 20)) {
+        *why = "batches of this size take the TMA pair";
+        return nullptr;
+    }
+    const size_t chunk = chunk_transforms(in, batch);
+    const KernelEntry<T>* k = pass_takes_kb(in, in.pass[0], chunk) ? in.pass[0].kcb : in.pass[0].kc;
+    if (!k) { *why = "the batched first pass tile has no c2r build"; return nullptr; }
+    const size_t rest = batch % chunk;
+    if (rest && !(pass_takes_kb(in, in.pass[0], rest) ? in.pass[0].kcb : in.pass[0].kc)) {
+        *why = "the last chunk's first pass tile has no c2r build";
+        return nullptr;
+    }
+    *why = "the batched first pass loads the half-spectra";
+    return k;
+}
+
+// Whether c2r of `batch` transforms folds the pre-processing (r2c.rs:764-780) into the loads of the inverse transform's first
+// pass under the current environment, and why (`why`: the rule that decided).  Fused: no scratch, one HBM round trip of N/2
+// complex values less.  PHASTFT_C2R_FUSE=0 keeps the separate sweep.  c2r_dev, the batched call and both describe functions
+// decide here, so they cannot disagree.
+template <typename T>
+bool c2r_fuses(const PlanR2c<T>* pl, size_t batch, const char** why) {
     const char* fuse_e = getenv("PHASTFT_C2R_FUSE");
     const Plan<T>& in = *pl->inner;
     const char* r = "the first pass loads the half-spectrum";
     bool fuse = false;
+    if (batch > 1) {
+        if (fuse_e && atoi(fuse_e) == 0) r = "PHASTFT_C2R_FUSE=0";
+        else fuse = c2r_batch_first_pass(in, batch, &r) != nullptr;
+        if (why) *why = r;
+        return fuse;
+    }
     if (fuse_e && atoi(fuse_e) == 0) r = "PHASTFT_C2R_FUSE=0";
     else if (in.num_passes < 2) r = "one-CTA inner plan";
     else if (!in.pass[0].kc) r = "the first pass tile has no c2r build";
@@ -1893,14 +1976,17 @@ bool c2r_fuses(const PlanR2c<T>* pl, const char** why) {
     return fuse;
 }
 
+// describe() (batch 1) and describe_batch(batch): the c2r path, the rule that decided and the c2r build of the first pass a call
+// of `batch` transforms runs.
 template <typename T>
-std::string r2c_description(const PlanR2c<T>* pl) {
+std::string r2c_description(const PlanR2c<T>* pl, size_t batch) {
     const char* why = nullptr;
-    const bool fuse = c2r_fuses(pl, &why);
+    const bool fuse = c2r_fuses(pl, batch, &why);
     const Plan<T>& in = *pl->inner;
     std::string s = "n=2^" + std::to_string(ilog2(pl->n)) + (sizeof(T) == 8 ? " f64" : " f32") + " r2c/c2r: c2r " +
                     (fuse ? "fused on load" : "separate sweep") + " (" + why + ") | c2r-in build: ";
-    const KernelEntry<T>* kc = in.num_passes >= 2 ? in.pass[0].kc : nullptr;
+    const char* unused = nullptr;
+    const KernelEntry<T>* kc = batch > 1 ? c2r_batch_first_pass(in, batch, &unused) : in.num_passes >= 2 ? in.pass[0].kc : nullptr;
     if (kc)
         s += std::string(kind_name(kc->kind)) + " R=" + std::to_string(kc->R) + " C=" + std::to_string(kc->C) + " NT=" +
              std::to_string(kc->NT) + " R1=" + std::to_string(kc->first_radix);
@@ -1917,7 +2003,7 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
     DeviceGuard g(pl->device);
     const size_t half = pl->n / 2;
     const Plan<T>& in = *pl->inner;
-    if (c2r_fuses(pl, nullptr)) {
+    if (c2r_fuses(pl, 1, nullptr)) {
         Io<T> io;
         io.in_re = d_ire; io.in_im = d_iim; io.in_il = 0; io.in_bstride = (long long)half;
         io.pre_tw2 = r2c_tw2(pl); io.pre_log2half = ilog2(half); io.pre_wc = pl->pre_wc;
@@ -1941,10 +2027,7 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
     RealParams<T> rp;
     memset(&rp, 0, sizeof(rp));
     rp.re = d_sre; rp.im = d_sim; rp.in_re = d_ire; rp.in_im = d_iim; rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
-    dim3 grid((unsigned)((half + 255) / 256), 1);
-    c2r_preprocess_kernel<T><<<grid, 256, 0, stream>>>(rp);
-    CUDA_TRY(cudaGetLastError());
-    note_launch({"C2R-PRE", (int)half, 0, 1, 256, 0, "plain", false});
+    if (int32_t st = launch_real(false, rp, half, 1, stream)) return st;
     // (2) inverse half-length c2c on the scratch (swap trick + 1/half, r2c.rs:782) with
     // (3) the re-interleave into the real output (r2c.rs:790-798) fused into the last store
     Io<T> io;
@@ -1957,6 +2040,124 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
         pl->scr_used = true;
     }
     return st;
+}
+
+// Grows the plan-owned c2r scratch to `elems` per array (batched sweeps).  Caller holds pl->mu.  The new arrays are allocated
+// before the old ones are released, so a failed allocation leaves the plan as it was.
+template <typename T>
+int32_t grow_r2c_scratch(const PlanR2c<T>* pl, size_t elems) {
+    if (pl->scr_elems >= elems) return PHASTFT_OK;
+    T* re = nullptr;
+    T* im = nullptr;
+    if (cudaMalloc(&re, elems * sizeof(T)) != cudaSuccess || cudaMalloc(&im, elems * sizeof(T)) != cudaSuccess) {
+        (void)cudaGetLastError();
+        if (re) cudaFree(re);
+        return fail(PHASTFT_ERR_CUDA, "cudaMalloc of the plan's c2r scratch for " + std::to_string(elems) + " elements failed");
+    }
+    CUDA_TRY(cudaDeviceSynchronize());   // every earlier user of the old scratch, on any stream, is done
+    cudaFree(pl->d_scr_re);
+    cudaFree(pl->d_scr_im);
+    pl->d_scr_re = re; pl->d_scr_im = im; pl->scr_elems = elems;
+    return PHASTFT_OK;
+}
+
+// Batched r2c: member b reads in_stride * b .. + N reals and writes N/2 + 1 bins at out_stride * b.  Batch 1 is r2c_dev.
+template <typename T>
+int32_t r2c_batch_dev(const PlanR2c<T>* pl, const T* d_in, size_t in_stride, T* d_ore, T* d_oim, size_t out_stride, size_t batch,
+                      cudaStream_t stream) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (!d_in) return fail(PHASTFT_ERR_INVALID_ARG, "d_input == NULL");
+    if (!d_ore) return fail(PHASTFT_ERR_INVALID_ARG, "d_out_re == NULL");
+    if (!d_oim) return fail(PHASTFT_ERR_INVALID_ARG, "d_out_im == NULL");
+    const size_t n = pl->n, half = n / 2;
+    if (in_stride < n || in_stride % 2)
+        return fail(PHASTFT_ERR_INVALID_ARG, "in_stride must be even and >= N = " + std::to_string(n) + " (got " + std::to_string(in_stride) + ")");
+    if (out_stride < half + 1)
+        return fail(PHASTFT_ERR_INVALID_ARG, "out_stride must be >= N/2 + 1 = " + std::to_string(half + 1) + " (got " + std::to_string(out_stride) + ")");
+    if (int32_t st = check_pair_alignment(d_in, "d_input")) return st;
+    if (batch == 0) return PHASTFT_OK;
+    if (batch == 1) return r2c_dev(pl, d_in, d_ore, d_oim, stream);
+    DeviceGuard g(pl->device);
+    Io<T> io;
+    io.in_re = d_in; io.in_im = nullptr; io.in_il = 1; io.in_bstride = (long long)(in_stride / 2);
+    io.out_re = d_ore; io.out_im = d_oim; io.out_il = 0; io.out_bstride = (long long)out_stride;
+    if (int32_t st = run_c2c(*pl->inner, io, batch, T(1), stream)) return st;
+    RealParams<T> rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.re = d_ore; rp.im = d_oim; rp.bstride = (long long)out_stride; rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
+    return launch_real(true, rp, half / 2 + 1, batch, stream);
+}
+
+// Batched c2r: member b reads N/2 + 1 bins at in_stride * b and writes N reals at out_stride * b.  Caller scratch holds
+// batch * N/2 elements per array, dense.  Batch 1 is c2r_dev.
+template <typename T>
+int32_t c2r_batch_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, size_t in_stride, T* d_out, size_t out_stride, T* d_sre,
+                      T* d_sim, size_t batch, cudaStream_t stream) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (!d_ire) return fail(PHASTFT_ERR_INVALID_ARG, "d_in_re == NULL");
+    if (!d_iim) return fail(PHASTFT_ERR_INVALID_ARG, "d_in_im == NULL");
+    if (!d_out) return fail(PHASTFT_ERR_INVALID_ARG, "d_output == NULL");
+    if ((d_sre == nullptr) != (d_sim == nullptr)) return fail(PHASTFT_ERR_INVALID_ARG, "pass both scratch arrays (d_scratch_re, d_scratch_im) or neither");
+    const size_t n = pl->n, half = n / 2;
+    if (in_stride < half + 1)
+        return fail(PHASTFT_ERR_INVALID_ARG, "in_stride must be >= N/2 + 1 = " + std::to_string(half + 1) + " (got " + std::to_string(in_stride) + ")");
+    if (out_stride < n || out_stride % 2)
+        return fail(PHASTFT_ERR_INVALID_ARG, "out_stride must be even and >= N = " + std::to_string(n) + " (got " + std::to_string(out_stride) + ")");
+    if (int32_t st = check_pair_alignment(d_out, "d_output")) return st;
+    if (batch == 0) return PHASTFT_OK;
+    if (batch == 1) return c2r_dev(pl, d_ire, d_iim, d_out, d_sre, d_sim, stream);
+    DeviceGuard g(pl->device);
+    Io<T> io;
+    io.out_re = d_out; io.out_im = nullptr; io.out_il = 2; io.out_bstride = (long long)(out_stride / 2);
+    if (c2r_fuses(pl, batch, nullptr)) {
+        io.in_re = d_ire; io.in_im = d_iim; io.in_il = 0; io.in_bstride = (long long)in_stride;
+        io.pre_tw2 = r2c_tw2(pl); io.pre_log2half = ilog2(half); io.pre_wc = pl->pre_wc; io.pre_wc_b = pl->pre_wc_b;
+        return run_c2c(*pl->inner, io, batch, T(1) / (T)half, stream);
+    }
+    std::unique_lock<std::mutex> lock(pl->mu, std::defer_lock);
+    bool own_scratch = false, capturing = false;
+    if (!d_sre) {
+        // the plan-owned scratch, grown to batch * N/2 (synchronising; an error while the stream is being captured)
+        lock.lock();
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+        capturing = cap != cudaStreamCaptureStatusNone;
+        if (pl->scr_elems < batch * half) {
+            if (capturing)
+                return fail(PHASTFT_ERR_INVALID_ARG, "the plan's c2r scratch is too small for this batch and the stream is being captured: "
+                                                     "call phastft_plan_r2c_*_reserve(batch) before capturing");
+            if (int32_t st = grow_r2c_scratch(pl, batch * half)) return st;
+        }
+        d_sre = pl->d_scr_re; d_sim = pl->d_scr_im;
+        own_scratch = true;
+        if (!capturing && pl->scr_used && pl->scr_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, pl->scr_free, 0));
+    }
+    RealParams<T> rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.re = d_sre; rp.im = d_sim; rp.bstride = (long long)half;
+    rp.in_re = d_ire; rp.in_im = d_iim; rp.in_bstride = (long long)in_stride;
+    rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
+    if (int32_t st = launch_real(false, rp, half, batch, stream)) return st;
+    io.in_re = d_sim; io.in_im = d_sre; io.in_il = 0; io.in_bstride = (long long)half;
+    int32_t st = run_c2c(*pl->inner, io, batch, T(1) / (T)half, stream);
+    if (st == PHASTFT_OK && own_scratch && !capturing) {
+        CUDA_TRY(cudaEventRecord(pl->scr_free, stream));
+        pl->scr_last_stream = stream;
+        pl->scr_used = true;
+    }
+    return st;
+}
+
+// Every allocation a batched call of `batch` would make: the inner plan's workspace, and the plan-owned c2r scratch when that
+// batch's c2r takes the sweep.
+template <typename T>
+int32_t r2c_reserve(const PlanR2c<T>* pl, size_t batch) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (int32_t st = plan_reserve(pl->inner, batch)) return st;
+    if (batch <= 1 || c2r_fuses(pl, batch, nullptr)) return PHASTFT_OK;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->mu);
+    return grow_r2c_scratch(pl, batch * (pl->n / 2));
 }
 
 template <typename T>
@@ -2200,8 +2401,27 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     size_t phastft_plan_r2c_##SFX##_size(const phastft_plan_r2c_##SFX* p) { return p ? AS_CR2C(T, p)->n : 0; }          \
     const char* phastft_plan_r2c_##SFX##_describe(const phastft_plan_r2c_##SFX* p) {                                    \
         if (!p) return "";                                                                                              \
-        g_r2c_desc_text = r2c_description<T>(AS_CR2C(T, p));                                                            \
+        g_r2c_desc_text = r2c_description<T>(AS_CR2C(T, p), 1);                                                         \
         return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
+    const char* phastft_plan_r2c_##SFX##_describe_batch(const phastft_plan_r2c_##SFX* p, size_t batch) {                \
+        if (!p) return "";                                                                                              \
+        g_r2c_desc_text = r2c_description<T>(AS_CR2C(T, p), batch);                                                     \
+        return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
+    int32_t phastft_plan_r2c_##SFX##_reserve(const phastft_plan_r2c_##SFX* p, size_t batch) {                           \
+        return r2c_reserve<T>(AS_CR2C(T, p), batch);                                                                    \
+    }                                                                                                                   \
+    int32_t phastft_r2c_##SFX##_batch_dev(const phastft_plan_r2c_##SFX* p, const T* in, size_t in_stride, T* ore,      \
+                                          T* oim, size_t out_stride, size_t batch, void* s) {                           \
+        launches_reset();                                                                                               \
+        return r2c_batch_dev<T>(AS_CR2C(T, p), in, in_stride, ore, oim, out_stride, batch, (cudaStream_t)s);            \
+    }                                                                                                                   \
+    int32_t phastft_c2r_##SFX##_batch_dev(const phastft_plan_r2c_##SFX* p, const T* ire, const T* iim,                 \
+                                          size_t in_stride, T* out, size_t out_stride, T* sre, T* sim, size_t batch,    \
+                                          void* s) {                                                                    \
+        launches_reset();                                                                                               \
+        return c2r_batch_dev<T>(AS_CR2C(T, p), ire, iim, in_stride, out, out_stride, sre, sim, batch, (cudaStream_t)s); \
     }                                                                                                                   \
     int32_t phastft_r2c_##SFX##_host(const phastft_plan_r2c_##SFX* p, const T* in, size_t lin, T* ore, size_t lore,    \
                                      T* oim, size_t loim) {                                                             \

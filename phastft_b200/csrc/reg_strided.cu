@@ -12,7 +12,9 @@ namespace phast {
 // (task-loop unrolling, twiddle derivation, register budget, thread count) are the ones that measured fastest for
 // that tile when it was tuned (not re-tuned on H100); push_entry also adds, for COL tiles, the MODE_C2R_IN build of the same kernel
 // (the first pass of the half-length inverse transform inside c2r, pre-processing folded into its loads) -- used on the tiles
-// the planner picks as the FIRST pass of a lone transform (a plan whose first pass has no such build keeps the separate sweep); variant 62 is the half-width 1024-row middle tile the planner asks
+// the planner picks as the FIRST pass of a lone transform (a plan whose first pass has no such build keeps the separate sweep);
+// push_entry_batch does the same for the first-pass tiles of batched calls (PassDesc::kb) of the inner plans of N = 2^13..2^31,
+// whose c2r build only batched c2r uses (PassDesc::kcb); variant 62 is the half-width 1024-row middle tile the planner asks
 // for by id.  The losing alternates of round 1 are no longer compiled.
 //   knob bits: 1 = unroll the task loops of the shared-memory stages, 2 = stage twiddles from 3 table loads +
 //   products, 4 = unroll the stage-1 task loop;  MINB = CTAs/SM the register budget is sized for.
@@ -30,26 +32,27 @@ void add_strided_kernels<PHAST_T, PHAST_KIND>(std::vector<KernelEntry<PHAST_T>>&
     v.push_back(make_entry_v<T, KIND, CN, 64, 0, 0, 0, 8, 8>());
     v.push_back(make_entry_v<T, KIND, CW, 128, 0, 0, 0, 8, 8>());
     v.push_back(make_entry_v<T, KIND, 2 * CW, 256, 0, 0, 0, 8, 8>());
-    v.push_back(make_entry_v<T, KIND, CN, 128, 0, 0, 0, 16, 8>());
+    push_entry_batch<T, KIND, CN, 128, 0, 0, 0, 16, 8>(v);
     push_entry<T, KIND, CW, 256, 0, 0, 0, 16, 8>(v);
     v.push_back(make_entry_v<T, KIND, 2 * CW, 256, 0, 0, 0, 16, 8>());
     // R = 256 as two radix-16 stages (one shared-memory exchange): faster as a first pass than
     // 4x8x8; 128 threads for the 64-byte-run f64 tile (128 tasks per stage)
     if constexpr (F64) {
-        v.push_back(make_entry_v<T, KIND, CN, 128, 0, 0, 0, 16, 16>());
+        push_entry_batch<T, KIND, CN, 128, 0, 0, 0, 16, 16>(v);
         push_entry<T, KIND, CW, 256, 0, 0, 0, 16, 16>(v);
         push_entry<T, KIND, CN, 256, 3, 2, 0, 8, 8, 8>(v);      // +20% over the plain build
         v.push_back(make_entry_v<T, KIND, CW, 256, 3, 2, 0, 8, 8, 8>());
         push_entry<T, KIND, CH, 256, 3, 2, 0, 8, 8, 8>(v);
-        v.push_back(make_entry_v<T, KIND, CN, 256, 0, 0, 0, 32, 32>());       // two radix-32 stages: faster at 2^20
+        // two radix-32 stages: faster at 2^20 (no c2r build: at 255 registers it spills, as the plain build does)
+        v.push_back(make_entry_v<T, KIND, CN, 256, 0, 0, 0, 32, 32>());
         push_entry<T, KIND, CH, 512, 0, 1, 0, 16, 8, 8>(v);
     } else {
-        v.push_back(make_entry_v<T, KIND, CN, 256, 0, 0, 0, 16, 16>());
+        push_entry_batch<T, KIND, CN, 256, 0, 0, 0, 16, 16>(v);
         push_entry<T, KIND, CW, 256, 0, 0, 0, 16, 16>(v);
         push_entry<T, KIND, CN, 256, 3, 2, 0, 8, 8, 8>(v);
         v.push_back(make_entry_v<T, KIND, CW, 256, 3, 2, 0, 8, 8, 8>());
         push_entry<T, KIND, CH, 256, 3, 2, 0, 8, 8, 8>(v);
-        v.push_back(make_entry_v<T, KIND, CN, 512, 0, 1, 0, 16, 8, 8>());
+        push_entry_batch<T, KIND, CN, 512, 0, 1, 0, 16, 8, 8>(v);
         push_entry<T, KIND, CH, 256, 0, 0, 0, 32, 32>(v);       // two radix-32 stages: faster at 2^20
     }
     // id 62: the 1024-row tile at half width (64 KB f64 / 32 KB f32) for interleaved intermediates, register budget

@@ -17,6 +17,8 @@ struct KernelEntry {
     int kind, R, C, NT, first_radix, stages, variant;
     int mode = 0;          // MODE_PLAIN, MODE_TMA_IN / MODE_BULK_IN (asynchronous tile input), MODE_C2R_IN (c2r pre-processing on load)
                            // or MODE_ROW_BULK (one-CTA batch kernel, tile in and out by cp.async.bulk)
+    bool batch_only = false;   // MODE_C2R_IN builds of the batch first-pass tiles: never a lone transform's c2r build (PassDesc::kc),
+                               // so adding one leaves every lone c2r on the path it had
     int rads[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the stage radices (the planner builds the one-CTA kernels' [i][m] stage-twiddle tables from them)
     size_t smem;
     const void* fn;        // fft_pass_kernel<...>; NULL for the passes of a cluster launch (they only exist inside it)
@@ -97,6 +99,16 @@ template <typename T, int KIND, int C, int NT, int VARIANT, int MINB, int ID, in
 void push_entry(std::vector<KernelEntry<T>>& v) {
     v.push_back(make_entry_v<T, KIND, C, NT, VARIANT, MINB, ID, Rs...>());
     if constexpr (KIND == KIND_COL) v.push_back(make_entry_async<T, KIND, C, NT, MODE_C2R_IN, VARIANT, MINB, ID, Rs...>());
+}
+// the same for a tile that is the first pass of batched calls only (PassDesc::kb): its c2r build serves batched c2r
+// (PassDesc::kcb) and is never looked up for a lone transform
+template <typename T, int KIND, int C, int NT, int VARIANT, int MINB, int ID, int... Rs>
+void push_entry_batch(std::vector<KernelEntry<T>>& v) {
+    v.push_back(make_entry_v<T, KIND, C, NT, VARIANT, MINB, ID, Rs...>());
+    if constexpr (KIND == KIND_COL) {
+        v.push_back(make_entry_async<T, KIND, C, NT, MODE_C2R_IN, VARIANT, MINB, ID, Rs...>());
+        v.back().batch_only = true;
+    }
 }
 
 template <typename T, int KIND, int C, int NT, int... Rs>

@@ -180,6 +180,37 @@ pub unsafe fn r2c_fft_f32_device(d_input: *const f32, d_out_re: *mut f32, d_out_
     check(ffi::phastft_r2c_f32_dev(planner.raw, d_input, d_out_re, d_out_im, stream));
 }
 /// # Safety
+/// Additive: `batch` r2c transforms in one call.  Member b reads N reals at `d_input + b * in_stride` (in_stride >= N, even)
+/// and writes N/2 + 1 bins at `d_out_* + b * out_stride` (out_stride >= N/2 + 1).  Batch 1 is [`r2c_fft_f64_device`].
+pub unsafe fn r2c_fft_f64_device_batch(d_input: *const f64, in_stride: usize, d_out_re: *mut f64, d_out_im: *mut f64, out_stride: usize,
+                                       batch: usize, planner: &PlannerR2c64, stream: *mut std::os::raw::c_void) {
+    check(ffi::phastft_r2c_f64_batch_dev(planner.raw, d_input, in_stride, d_out_re, d_out_im, out_stride, batch, stream));
+}
+
+/// Additive: `batch` c2r transforms in one call.  Member b reads N/2 + 1 bins at `d_in_* + b * in_stride` (in_stride >= N/2 + 1)
+/// and writes N reals at `d_output + b * out_stride` (out_stride >= N, even); `d_scratch_*` hold batch * N/2 each, dense, or are
+/// both null (the plan's own scratch).  Batch 1 is [`c2r_fft_f64_device`].
+pub unsafe fn c2r_fft_f64_device_batch(d_in_re: *const f64, d_in_im: *const f64, in_stride: usize, d_output: *mut f64, out_stride: usize,
+                                       batch: usize, planner: &PlannerR2c64, d_scratch_re: *mut f64, d_scratch_im: *mut f64,
+                                       stream: *mut std::os::raw::c_void) {
+    check(ffi::phastft_c2r_f64_batch_dev(planner.raw, d_in_re, d_in_im, in_stride, d_output, out_stride, d_scratch_re, d_scratch_im,
+                                         batch, stream));
+}
+
+/// As [`r2c_fft_f64_device_batch`].
+pub unsafe fn r2c_fft_f32_device_batch(d_input: *const f32, in_stride: usize, d_out_re: *mut f32, d_out_im: *mut f32, out_stride: usize,
+                                       batch: usize, planner: &PlannerR2c32, stream: *mut std::os::raw::c_void) {
+    check(ffi::phastft_r2c_f32_batch_dev(planner.raw, d_input, in_stride, d_out_re, d_out_im, out_stride, batch, stream));
+}
+
+/// As [`c2r_fft_f64_device_batch`].
+pub unsafe fn c2r_fft_f32_device_batch(d_in_re: *const f32, d_in_im: *const f32, in_stride: usize, d_output: *mut f32, out_stride: usize,
+                                       batch: usize, planner: &PlannerR2c32, d_scratch_re: *mut f32, d_scratch_im: *mut f32,
+                                       stream: *mut std::os::raw::c_void) {
+    check(ffi::phastft_c2r_f32_batch_dev(planner.raw, d_in_re, d_in_im, in_stride, d_output, out_stride, d_scratch_re, d_scratch_im,
+                                         batch, stream));
+}
+
 /// As [`c2r_fft_f64_device`].
 pub unsafe fn c2r_fft_f32_device(d_in_re: *const f32, d_in_im: *const f32, d_output: *mut f32, planner: &PlannerR2c32,
                                  d_scratch_re: *mut f32, d_scratch_im: *mut f32, stream: *mut std::os::raw::c_void) {
