@@ -69,6 +69,14 @@ template <> struct Api<double> {
     static void r2c_destroy(R2c* p) { phastft_plan_r2c_f64_destroy(p); }
     static int32_t r2c_host(const R2c* p, const double* in, std::size_t li, double* ore, std::size_t lre, double* oim, std::size_t lim) { return phastft_r2c_f64_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const double* ire, std::size_t lre, const double* iim, std::size_t lim, double* out, std::size_t lo, double* sre, std::size_t lsr, double* sim, std::size_t lsi) { return phastft_c2r_f64_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
+    using Any = phastft_plan_any_f64;
+    static int32_t any_create(std::size_t n, int dev, Any** o) { return phastft_plan_any_f64_create(n, dev, o); }
+    static void any_destroy(Any* p) { phastft_plan_any_f64_destroy(p); }
+    static std::size_t any_size(const Any* p) { return phastft_plan_any_f64_size(p); }
+    static const char* any_describe(const Any* p) { return phastft_plan_any_f64_describe(p); }
+    static int32_t any_reserve(const Any* p, std::size_t b) { return phastft_plan_any_f64_reserve(p, b); }
+    static int32_t any_dev(const Any* p, double* re, double* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f64_dev(p, re, im, d, b, st, s); }
+    static int32_t any_host(const Any* p, double* re, std::size_t lr, double* im, std::size_t li, int d) { return phastft_fft_any_f64_host(p, re, lr, im, li, d); }
 };
 template <> struct Api<float> {
     using Dit = phastft_plan_dit_f32; using R2c = phastft_plan_r2c_f32;
@@ -90,6 +98,14 @@ template <> struct Api<float> {
     static void r2c_destroy(R2c* p) { phastft_plan_r2c_f32_destroy(p); }
     static int32_t r2c_host(const R2c* p, const float* in, std::size_t li, float* ore, std::size_t lre, float* oim, std::size_t lim) { return phastft_r2c_f32_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const float* ire, std::size_t lre, const float* iim, std::size_t lim, float* out, std::size_t lo, float* sre, std::size_t lsr, float* sim, std::size_t lsi) { return phastft_c2r_f32_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
+    using Any = phastft_plan_any_f32;
+    static int32_t any_create(std::size_t n, int dev, Any** o) { return phastft_plan_any_f32_create(n, dev, o); }
+    static void any_destroy(Any* p) { phastft_plan_any_f32_destroy(p); }
+    static std::size_t any_size(const Any* p) { return phastft_plan_any_f32_size(p); }
+    static const char* any_describe(const Any* p) { return phastft_plan_any_f32_describe(p); }
+    static int32_t any_reserve(const Any* p, std::size_t b) { return phastft_plan_any_f32_reserve(p, b); }
+    static int32_t any_dev(const Any* p, float* re, float* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f32_dev(p, re, im, d, b, st, s); }
+    static int32_t any_host(const Any* p, float* re, std::size_t lr, float* im, std::size_t li, int d) { return phastft_fft_any_f32_host(p, re, lr, im, li, d); }
 };
 
 /// planner.rs:34-114
@@ -141,12 +157,40 @@ class PlannerR2c {
   private:
     typename Api<T>::R2c* raw_ = nullptr;
 };
+
+/// additive: a complex FFT of any length (a power of two runs the c2c plan; any other length up to 2^29 - 1, Bluestein's algorithm)
+template <typename T>
+class PlannerAny {
+  public:
+    explicit PlannerAny(std::size_t num_points, int device = 0) { check(Api<T>::any_create(num_points, device, &raw_)); }
+    ~PlannerAny() { if (raw_) Api<T>::any_destroy(raw_); }
+    PlannerAny(PlannerAny&& o) noexcept : raw_(o.raw_) { o.raw_ = nullptr; }
+    PlannerAny(const PlannerAny&) = delete;
+    PlannerAny& operator=(const PlannerAny&) = delete;
+    std::size_t num_points() const { return Api<T>::any_size(raw_); }
+    /// "power of two" or "Bluestein M=2^m", then the inner plan's description
+    std::string describe() const { return Api<T>::any_describe(raw_); }
+    /// make every allocation a call of `batch` transforms would make now
+    void reserve(std::size_t batch) const { check(Api<T>::any_reserve(raw_, batch)); }
+    /// in place on planar host vectors; forward unscaled, reverse scaled by 1/N
+    void fft(std::vector<T>& reals, std::vector<T>& imags, Direction d) const {
+        check(Api<T>::any_host(raw_, reals.data(), reals.size(), imags.data(), imags.size(), (int)d));
+    }
+    /// `batch` transforms on device pointers, transform b at b * batch_stride; stream-ordered on `stream`
+    void fft_device(T* d_reals, T* d_imags, Direction d, std::size_t batch, std::size_t batch_stride, void* stream = nullptr) const {
+        check(Api<T>::any_dev(raw_, d_reals, d_imags, (int)d, batch, batch_stride, stream));
+    }
+  private:
+    typename Api<T>::Any* raw_ = nullptr;
+};
 }  // namespace detail
 
 using PlannerDit64 = detail::PlannerDit<double>;
 using PlannerDit32 = detail::PlannerDit<float>;
 using PlannerR2c64 = detail::PlannerR2c<double>;
 using PlannerR2c32 = detail::PlannerR2c<float>;
+using PlannerAny64 = detail::PlannerAny<double>;
+using PlannerAny32 = detail::PlannerAny<float>;
 
 // ---- c2c (lib.rs:143-226, algorithms/dit.rs:263,338): in place on planar vectors -----------------------
 inline void fft_64_dit_with_planner_and_opts(std::vector<double>& reals, std::vector<double>& imags, Direction d, const PlannerDit64& p, const Options&) {

@@ -46,7 +46,7 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * by "; ".  Each entry reads "<kind> R=<rows> C=<columns> NT=<threads> v<variant> <mode>[ pdl]": kind COL / TRANS (strided
  * passes), ROW (one CTA per transform), CLUSTER (both passes in one cluster launch: R=<R1>x<R2>, K=<CTAs per cluster>),
  * PIPE (both passes in one pipelined launch: R=<R1>x<R2>), R2C-UNTANGLE / C2R-PRE (the real transforms' elementwise
- * kernels); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * kernels), CHIRP-PRE / CHIRP-MUL / CHIRP-POST (the any-length transform's elementwise kernels: R=<M>, C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
@@ -262,6 +262,42 @@ PHASTFT_API int32_t phastft_c2r_f64_batch_dev(const phastft_plan_r2c_f64* plan, 
 PHASTFT_API int32_t phastft_c2r_f32_batch_dev(const phastft_plan_r2c_f32* plan, const float* d_in_re, const float* d_in_im,
                                               size_t in_stride, float* d_output, size_t out_stride, float* d_scratch_re,
                                               float* d_scratch_im, size_t batch, void* stream);
+
+/* ---- complex FFTs of any length (the reference accepts powers of two only) -------------------------------------------
+ * n >= 1.  A power of two runs the n-point c2c plan exactly as phastft_fft_dit_*_dev does (same results, same launches).
+ * Any other n up to 2^29 - 1 uses Bluestein's chirp-z algorithm: with w[j] = exp(-pi i (j^2 mod 2n) / n),
+ * X[k] = w[k] sum_j (x[j] w[j]) conj(w[k - j]), a circular convolution of length M = 2^ceil(log2(2n - 1)) computed by two
+ * forward M-point c2c transforms of the library between three elementwise kernels (CHIRP-PRE, CHIRP-MUL, CHIRP-POST in
+ * phastft_last_launches).  The plan owns the chirp, the transform of the convolution kernel (computed once in f64) and a
+ * workspace of batch * M complex values.  Any other n returns PHASTFT_ERR_INVALID_ARG before the device is touched.
+ * Semantics of the fft_dit entry points: planar, in place, natural order, forward unscaled, reverse scaled by 1/n. */
+typedef struct phastft_plan_any_f64 phastft_plan_any_f64;
+typedef struct phastft_plan_any_f32 phastft_plan_any_f32;
+PHASTFT_API int32_t phastft_plan_any_f64_create(size_t n, int device, phastft_plan_any_f64** out);
+PHASTFT_API int32_t phastft_plan_any_f32_create(size_t n, int device, phastft_plan_any_f32** out);
+PHASTFT_API void phastft_plan_any_f64_destroy(phastft_plan_any_f64* plan);
+PHASTFT_API void phastft_plan_any_f32_destroy(phastft_plan_any_f32* plan);
+PHASTFT_API size_t phastft_plan_any_f64_size(const phastft_plan_any_f64* plan);
+PHASTFT_API size_t phastft_plan_any_f32_size(const phastft_plan_any_f32* plan);
+/* "n=1000 f64 any: Bluestein M=2^11 | inner: n=2^11 f64: ..." or "n=2^20 f64 any: power of two | inner: n=2^20 f64: ..." */
+PHASTFT_API const char* phastft_plan_any_f64_describe(const phastft_plan_any_f64* plan);
+PHASTFT_API const char* phastft_plan_any_f32_describe(const phastft_plan_any_f32* plan);
+/* Makes every allocation a call of `batch` transforms would make now: the inner plan's workspace and this plan's batch * M.
+ * A call that would grow either while its stream is being captured into a CUDA graph returns PHASTFT_ERR_INVALID_ARG. */
+PHASTFT_API int32_t phastft_plan_any_f64_reserve(const phastft_plan_any_f64* plan, size_t batch);
+PHASTFT_API int32_t phastft_plan_any_f32_reserve(const phastft_plan_any_f32* plan, size_t batch);
+/* Device-resident, asynchronous on `stream`: `batch` transforms, transform b at d_re + b * batch_stride (batch_stride >= n
+ * when batch > 1).  batch == 0 launches nothing.  NULL pointers and bad directions return PHASTFT_ERR_INVALID_ARG before any
+ * launch.  Allocates only when the plan's workspace must grow (synchronising). */
+PHASTFT_API int32_t phastft_fft_any_f64_dev(const phastft_plan_any_f64* plan, double* d_reals, double* d_imags, int direction,
+                                            size_t batch, size_t batch_stride, void* stream);
+PHASTFT_API int32_t phastft_fft_any_f32_dev(const phastft_plan_any_f32* plan, float* d_reals, float* d_imags, int direction,
+                                            size_t batch, size_t batch_stride, void* stream);
+/* Host slices, synchronous, in place: len_re != len_im -> PHASTFT_ERR_LEN_MISMATCH, length != n -> PHASTFT_ERR_PLAN_MISMATCH. */
+PHASTFT_API int32_t phastft_fft_any_f64_host(const phastft_plan_any_f64* plan, double* reals, size_t len_re, double* imags,
+                                             size_t len_im, int direction);
+PHASTFT_API int32_t phastft_fft_any_f32_host(const phastft_plan_any_f32* plan, float* reals, size_t len_re, float* imags,
+                                             size_t len_im, int direction);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

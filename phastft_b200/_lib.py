@@ -106,6 +106,13 @@ SIGNATURES = {
     "phastft_c2r_{s}_dev": ([_vp, _vp, _vp, _vp, _vp, _vp, _vp], _i32),
     "phastft_r2c_{s}_batch_dev": ([_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp], _i32),
     "phastft_c2r_{s}_batch_dev": ([_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp], _i32),
+    "phastft_plan_any_{s}_create": ([_sz, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_any_{s}_destroy": ([_vp], None),
+    "phastft_plan_any_{s}_size": ([_vp], _sz),
+    "phastft_plan_any_{s}_describe": ([_vp], C.c_char_p),
+    "phastft_plan_any_{s}_reserve": ([_vp, _sz], _i32),
+    "phastft_fft_any_{s}_dev": ([_vp, _vp, _vp, _ci, _sz, _sz, _vp], _i32),
+    "phastft_fft_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _ci], _i32),
 }
 def check(code: int):
     if code != OK:

@@ -39,6 +39,7 @@ __all__ = [
     "c2r_fft_f32_with_planner_and_scratch",
     "fft_dit_batch", "fft_dit_batch_sharded", "host_register", "host_unregister",
     "r2c_batch", "c2r_batch",
+    "PlannerAny64", "PlannerAny32", "fft_64_any_with_planner", "fft_32_any_with_planner", "fft_any_batch",
 ]
 
 
@@ -222,6 +223,50 @@ class PlannerR2c64(_PlannerR2c):
 
 
 class PlannerR2c32(_PlannerR2c):
+    _sfx, _dtype = "f32", np.float32
+
+
+class _PlannerAny:
+    _sfx = ""
+    _dtype = None
+
+    def __init__(self, num_points: int, device: int = 0):
+        """A complex FFT of any length num_points >= 1 (the reference accepts powers of two only): a power of two runs the
+        c2c plan as it is, any other length up to 2^29 - 1 Bluestein's algorithm over a power-of-two plan.  Other lengths
+        raise PhastFTPanic(13) before the device is touched."""
+        self._h = C.c_void_p()
+        self.device = int(device)
+        check(fn("phastft_plan_any_{s}_create", self._sfx)(int(num_points), self.device, C.byref(self._h)))
+        self.num_points = int(num_points)
+
+    @classmethod
+    def new(cls, num_points: int, device: int = 0):
+        return cls(num_points, device)
+
+    def describe(self) -> str:
+        """"power of two" or "Bluestein M=2^m" (the convolution length), then the inner plan's describe()."""
+        return fn("phastft_plan_any_{s}_describe", self._sfx)(self._h).decode()
+
+    def reserve(self, batch: int) -> None:
+        """Make every allocation a call of `batch` transforms would make now (otherwise the first larger call makes them,
+        synchronising the device -- an error inside a CUDA-graph capture)."""
+        check(fn("phastft_plan_any_{s}_reserve", self._sfx)(self._h, int(batch)))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._h = None
+            try:
+                fn("phastft_plan_any_{s}_destroy", self._sfx)(h)
+            except (AttributeError, TypeError):      # interpreter shutdown: the module globals are already gone
+                pass
+
+
+class PlannerAny64(_PlannerAny):
+    _sfx, _dtype = "f64", np.float64
+
+
+class PlannerAny32(_PlannerAny):
     _sfx, _dtype = "f32", np.float32
 
 
@@ -619,3 +664,46 @@ def c2r_batch(in_re, in_im, out, planner, batch: int, in_stride: int | None = No
                                                         psr, psi, int(batch), _torch_stream(out)))
     if work is not out:
         out.copy_(work)
+
+
+# ----------------------------------------------------------------------------------------------
+# complex FFTs of any length (the reference accepts powers of two only)
+# ----------------------------------------------------------------------------------------------
+def _fft_any_with_planner(sfx, dtype, reals, imags, direction, planner):
+    if planner._sfx != sfx:
+        raise TypeError("planner precision does not match the function")
+    if _is_torch(reals):
+        pr, nr = _torch_ptr(reals, dtype)
+        pi, ni = _torch_ptr(imags, dtype)
+        if nr != ni:
+            raise PhastFTPanic(1)
+        if nr != planner.num_points:
+            raise PhastFTPanic(3)
+        check(fn("phastft_fft_any_{s}_dev", sfx)(planner._h, pr, pi, int(direction), 1, nr, _torch_stream(reals)))
+    else:
+        pr, nr = _np_ptr(reals, dtype, True)
+        pi, ni = _np_ptr(imags, dtype, True)
+        check(fn("phastft_fft_any_{s}_host", sfx)(planner._h, pr, nr, pi, ni, int(direction)))
+
+
+def fft_64_any_with_planner(reals, imags, direction: Direction, planner: PlannerAny64) -> None:
+    """fft_64_dit_with_planner for any length: numpy arrays (synchronous) or torch CUDA tensors (torch's current stream)."""
+    _fft_any_with_planner("f64", np.float64, reals, imags, direction, planner)
+
+
+def fft_32_any_with_planner(reals, imags, direction: Direction, planner: PlannerAny32) -> None:
+    _fft_any_with_planner("f32", np.float32, reals, imags, direction, planner)
+
+
+def fft_any_batch(reals, imags, direction: Direction, planner, batch: int, batch_stride: int | None = None) -> None:
+    """fft_dit_batch for any length: `batch` signals of planner.num_points, transform b at offset b * batch_stride of the planar
+    torch CUDA tensors."""
+    n = planner.num_points
+    stride = n if batch_stride is None else int(batch_stride)
+    pr, nr = _torch_ptr(reals, planner._dtype)
+    pi, ni = _torch_ptr(imags, planner._dtype)
+    if nr != ni:
+        raise PhastFTPanic(1)
+    _check_batch_len("tensors", nr, batch, stride, n)
+    check(fn("phastft_fft_any_{s}_dev", planner._sfx)(planner._h, pr, pi, int(direction), int(batch), stride,
+                                                      _torch_stream(reals)))

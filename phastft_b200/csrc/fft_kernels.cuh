@@ -906,4 +906,119 @@ __global__ void __launch_bounds__(256) c2r_preprocess_kernel(const __grid_consta
     zim[k] = zx_im + zy_re;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Bluestein's chirp-z algorithm (any N, phastft_fft_any_*): X[k] = w[k] sum_n (x[n] w[n]) conj(w[k-n]), w[j] =
+// exp(-pi i (j^2 mod 2N) / N), a circular convolution of length M = 2^ceil(log2(2N - 1)) done with two forward M-point
+// transforms in place on an interleaved workspace of M complex values per member:
+//   CHIRP-PRE   a[m] = x[m] w[m] (m < N), 0 (N <= m < M)
+//   CHIRP-MUL   A[k] <- conj(A[k] Bh[k]),  Bh = FFT_M(b) / M,  b[m] = conj(w[|m|]) on the circle
+//   CHIRP-POST  X[k] = scale * w[k] conj(C[k]) (k < N)
+// (the conjugation makes the second forward transform an inverse one: ifft(Y) = conj(fft(conj Y)) / M).  Each thread moves 16
+// bytes of the interleaved side (one complex f64, two complex f32) in one access; grids are member-major like the r2c ones.
+// ---------------------------------------------------------------------------------------------
+template <typename T> struct Cx16;
+template <> struct Cx16<double> {
+    static constexpr int V = 1;
+    using vec = double2;
+    __device__ static void unpack(const double2& q, double2* c) { c[0] = q; }
+    __device__ static double2 pack(const double2* c) { return c[0]; }
+};
+template <> struct Cx16<float> {
+    static constexpr int V = 2;
+    using vec = float4;
+    __device__ static void unpack(const float4& q, float2* c) { c[0] = make_float2(q.x, q.y); c[1] = make_float2(q.z, q.w); }
+    __device__ static float4 pack(const float2* c) { return make_float4(c[0].x, c[0].y, c[1].x, c[1].y); }
+};
+
+template <typename T>
+struct ChirpParams {
+    const T* in_re;                // CHIRP-PRE: the caller's planar input (re / im swapped for the reverse direction)
+    const T* in_im;
+    T* out_re;                     // CHIRP-POST: the caller's planar output (swapped like the input)
+    T* out_im;
+    cx<T>* ws;                     // members x M interleaved complex
+    const cx<T>* chirp;            // w[0 .. N), padded with zeros to a multiple of Cx16<T>::V
+    const cx<T>* bhat;             // FFT_M(b) / M
+    long long bstride;             // elements between members of the caller's arrays
+    long long n;
+    int log2m;
+    unsigned blocks_per_member;    // the grid is members x blocks_per_member blocks, member-major
+    T scale;                       // CHIRP-POST: 1 forward, 1/N reverse
+};
+
+// index of this thread's first complex value in its member, and the member
+template <typename T>
+__device__ __forceinline__ long long chirp_index(const ChirpParams<T>& p, unsigned& mb) {
+    mb = blockIdx.x / p.blocks_per_member;
+    return ((long long)(blockIdx.x - mb * p.blocks_per_member) * blockDim.x + threadIdx.x) * Cx16<T>::V;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) chirp_pre_kernel(const __grid_constant__ ChirpParams<T> p) {
+    using P = Cx16<T>;
+    unsigned mb;
+    const long long m0 = chirp_index(p, mb);
+    const long long M = 1LL << p.log2m;
+    if (m0 >= M) return;
+    cx<T> a[P::V];
+    if (m0 < p.n) {
+        cx<T> w[P::V];
+        P::unpack(reinterpret_cast<const typename P::vec*>(p.chirp)[m0 / P::V], w);
+        const T* re = p.in_re + (long long)mb * p.bstride;
+        const T* im = p.in_im + (long long)mb * p.bstride;
+#pragma unroll
+        for (int j = 0; j < P::V; ++j)
+            a[j] = m0 + j < p.n ? cmul<T>(make_cx<T>(re[m0 + j], im[m0 + j]), w[j]) : make_cx<T>(T(0), T(0));
+    } else {
+#pragma unroll
+        for (int j = 0; j < P::V; ++j) a[j] = make_cx<T>(T(0), T(0));
+    }
+    reinterpret_cast<typename P::vec*>(p.ws + ((long long)mb << p.log2m))[m0 / P::V] = P::pack(a);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) chirp_mul_kernel(const __grid_constant__ ChirpParams<T> p) {
+    using P = Cx16<T>;
+    unsigned mb;
+    const long long k0 = chirp_index(p, mb);
+    if (k0 >= (1LL << p.log2m)) return;
+    typename P::vec* ws = reinterpret_cast<typename P::vec*>(p.ws + ((long long)mb << p.log2m)) + k0 / P::V;
+    cx<T> a[P::V], b[P::V];
+    P::unpack(*ws, a);
+    P::unpack(reinterpret_cast<const typename P::vec*>(p.bhat)[k0 / P::V], b);
+#pragma unroll
+    for (int j = 0; j < P::V; ++j) {
+        const cx<T> y = cmul<T>(a[j], b[j]);
+        a[j] = make_cx<T>(y.x, -y.y);
+    }
+    *ws = P::pack(a);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) chirp_post_kernel(const __grid_constant__ ChirpParams<T> p) {
+    using P = Cx16<T>;
+    unsigned mb;
+    const long long k0 = chirp_index(p, mb);
+    if (k0 >= p.n) return;
+    cx<T> c[P::V], w[P::V];
+    P::unpack(reinterpret_cast<const typename P::vec*>(p.ws + ((long long)mb << p.log2m))[k0 / P::V], c);
+    P::unpack(reinterpret_cast<const typename P::vec*>(p.chirp)[k0 / P::V], w);
+    T* re = p.out_re + (long long)mb * p.bstride;
+    T* im = p.out_im + (long long)mb * p.bstride;
+#pragma unroll
+    for (int j = 0; j < P::V; ++j) {
+        if (k0 + j >= p.n) break;
+        const cx<T> x = cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y));
+        re[k0 + j] = x.x * p.scale;
+        im[k0 + j] = x.y * p.scale;
+    }
+}
+
+// Plan time, f32 plans: Bh rounded to T from its f64 transform.
+template <typename T>
+__global__ void __launch_bounds__(256) chirp_narrow_kernel(const double2* __restrict__ in, cx<T>* __restrict__ out, long long count) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (long long)gridDim.x * blockDim.x)
+        out[i] = make_cx<T>((T)in[i].x, (T)in[i].y);
+}
+
 }  // namespace phast

@@ -21,6 +21,8 @@
 #include <string>
 #include <algorithm>
 #include <functional>
+#include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/phastft_cuda.h"
@@ -175,6 +177,34 @@ void root_of_unity(uint64_t k, uint64_t n, double& re, double& im) {
         case 5: cs(eighth - rem, c, s); co = -s; si = -c; break;
         case 6: cs(rem, c, s); co = s; si = -c; break;
         default: cs(eighth - rem, c, s); co = c; si = -s; break;
+    }
+    re = (double)co;
+    im = (double)(-si);
+    if (re == 0.0) re = 0.0;
+    if (im == 0.0) im = 0.0;
+}
+
+// W_n^k = exp(-2*pi*i*k/n) for any n >= 1 (k * 8 < 2^64): root_of_unity's octant reduction, with the octant found in integers
+// from 8k = oct * n + rem, so the angle left for cosl / sinl is (pi/4) * rem / n or (pi/4) * (n - rem) / n.
+void root_of_unity_any(uint64_t k, uint64_t n, double& re, double& im) {
+    k %= n;
+    const uint64_t oct = 8 * k / n, rem = 8 * k % n;
+    auto cs = [&](uint64_t j, long double& c, long double& s) {
+        if (j == 0) { c = 1.0L; s = 0.0L; return; }
+        if (j == n) { c = s = 0.70710678118654752440084436210484903928L; return; }
+        long double a = 0.25L * 3.14159265358979323846264338327950288L * (long double)j / (long double)n;
+        c = cosl(a); s = sinl(a);
+    };
+    long double c, s, co, si;
+    switch (oct) {
+        case 0: cs(rem, c, s); co = c; si = s; break;
+        case 1: cs(n - rem, c, s); co = s; si = c; break;
+        case 2: cs(rem, c, s); co = -s; si = c; break;
+        case 3: cs(n - rem, c, s); co = -c; si = s; break;
+        case 4: cs(rem, c, s); co = -c; si = -s; break;
+        case 5: cs(n - rem, c, s); co = -s; si = -c; break;
+        case 6: cs(rem, c, s); co = s; si = -c; break;
+        default: cs(n - rem, c, s); co = c; si = -s; break;
     }
     re = (double)co;
     im = (double)(-si);
@@ -2238,6 +2268,275 @@ int32_t oneshot_r2c_plan(OneShotCache<PlanR2c<T>>& c, size_t n, int device, Plan
     return PHASTFT_OK;
 }
 
+// =================================================================================================
+// any length: Bluestein's chirp-z algorithm over the power-of-two plans (the CHIRP-* kernels, fft_kernels.cuh)
+// =================================================================================================
+// The largest length that is not a power of two: its convolution length M = 2^ceil(log2(2N - 1)) is 2^30, the largest
+// power-of-two plan.
+constexpr size_t ANY_MAX_N = (size_t(1) << 29) - 1;
+
+template <typename T>
+struct PlanAny {
+    size_t n = 0;
+    int log2m = 0;                     // 0: N is a power of two and `inner` is the N-point plan, run as it is
+    int device = 0;
+    Plan<T>* inner = nullptr;          // the M-point plan of both convolution transforms
+    cx<T>* chirp = nullptr;            // w[0 .. N), zero-padded to a multiple of Cx16<T>::V
+    cx<T>* bhat = nullptr;             // FFT_M(b) / M, computed in f64
+    mutable std::mutex mu;             // the workspace and the host staging
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then mu)
+    mutable cx<T>* ws = nullptr;       // ws_members x M interleaved complex
+    mutable size_t ws_members = 0;
+    mutable cudaEvent_t ws_free = nullptr;   // orders workspace reuse across streams (like Plan::ws_free)
+    mutable cudaStream_t ws_last_stream = nullptr;
+    mutable bool ws_used = false;
+    mutable T* stage_re = nullptr;     // host-API staging: N each
+    mutable T* stage_im = nullptr;
+    std::string description;
+    ~PlanAny() {
+        DeviceGuard g(device);
+        if (ws_free) cudaEventDestroy(ws_free);
+        for (void* p : {(void*)chirp, (void*)bhat, (void*)ws, (void*)stage_re, (void*)stage_im})
+            if (p) cudaFree(p);
+        delete inner;
+    }
+};
+
+// w[j] = exp(-pi i (j^2 mod 2N) / N) for j in [s, s + count): the phase is reduced exactly in integers (j^2 < 2^58 for
+// j < 2^29) and evaluated in long double with octant symmetry.  Spread over the host's cores: 2^29 entries take minutes on one.
+void chirp_table(size_t n, size_t s, size_t count, double2* w) {
+    auto work = [=](size_t t, size_t step) {
+        for (size_t i = t; i < count; i += step) {
+            const uint64_t j = s + i;
+            root_of_unity_any(j * j % (2 * n), 2 * n, w[i].x, w[i].y);
+        }
+    };
+    const size_t nt = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), 64);
+    if (count < 8192 || nt == 1) { work(0, 1); return; }
+    std::vector<std::thread> th;
+    for (size_t t = 0; t < nt; ++t) th.emplace_back(work, t, nt);
+    for (std::thread& x : th) x.join();
+}
+
+template <typename T>
+int32_t build_plan_any(size_t n, int device, PlanAny<T>** out) {
+    if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
+    *out = nullptr;
+    if (n == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n must be >= 1");
+    const bool pow2 = is_pow2(n);
+    if (!pow2 && n > ANY_MAX_N)
+        return fail(PHASTFT_ERR_INVALID_ARG, "n = " + std::to_string(n) + " is not a power of two and above 2^29 - 1 (its convolution "
+                                             "length 2^ceil(log2(2N - 1)) would exceed 2^30)");
+    std::unique_ptr<PlanAny<T>> pl(new PlanAny<T>());
+    pl->n = n; pl->device = device;
+    const char* prec = sizeof(T) == 8 ? " f64" : " f32";
+    if (pow2) {
+        if (int32_t st = build_plan<T>(n, device, &pl->inner)) return st;
+        pl->description = "n=2^" + std::to_string(ilog2(n)) + prec + " any: power of two | inner: " + pl->inner->description;
+        *out = pl.release();
+        return PHASTFT_OK;
+    }
+    int lm = 0;
+    while ((size_t(1) << lm) < 2 * n - 1) ++lm;
+    const size_t M = size_t(1) << lm;
+    pl->log2m = lm;
+    if (int32_t st = build_plan<T>(M, device, &pl->inner)) return st;
+    DeviceGuard g(device);
+    // w in T for the kernels, and b[m] = conj(w[|m|]) on the circle of M points in f64 (0 where |m| >= N), built chunk by chunk
+    constexpr size_t V = Cx16<T>::V;
+    const size_t nc = (n + V - 1) / V * V;
+    CUDA_TRY(cudaMalloc(&pl->chirp, nc * sizeof(cx<T>)));
+    CUDA_TRY(cudaMemset(pl->chirp, 0, nc * sizeof(cx<T>)));
+    double2* b = nullptr;
+    CUDA_TRY(cudaMalloc(&b, M * sizeof(double2)));
+    std::unique_ptr<double2, void (*)(double2*)> b_owner(b, [](double2* p) { cudaFree(p); });
+    CUDA_TRY(cudaMemset(b, 0, M * sizeof(double2)));
+    const size_t CH = size_t(1) << 20;
+    std::vector<double2> w(std::min(CH, n)), rev(std::min(CH, n));
+    std::vector<cx<T>> wt(std::min(CH, n));
+    for (size_t s = 0; s < n; s += CH) {
+        const size_t cnt = std::min(CH, n - s);
+        chirp_table(n, s, cnt, w.data());
+        for (size_t i = 0; i < cnt; ++i) {
+            wt[i].x = (T)w[i].x; wt[i].y = (T)w[i].y;
+            w[i].y = -w[i].y;                                         // b[m] = conj(w[m])
+        }
+        CUDA_TRY(cudaMemcpy(pl->chirp + s, wt.data(), cnt * sizeof(cx<T>), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(b + s, w.data(), cnt * sizeof(double2), cudaMemcpyHostToDevice));
+        // b[M - m] = b[m] for 0 < m < N: m = s + cnt - 1 - i lands at M - m, ascending in i
+        const size_t lo = std::max<size_t>(s, 1), k = s + cnt - lo;
+        for (size_t i = 0; i < k; ++i) rev[i] = w[cnt - 1 - i];
+        if (k) CUDA_TRY(cudaMemcpy(b + (M - (s + cnt - 1)), rev.data(), k * sizeof(double2), cudaMemcpyHostToDevice));
+    }
+    CUDA_TRY(cudaDeviceSynchronize());
+    // Bh = FFT_M(b) / M in f64, in place (the scale is a power of two: exact): with the inner plan for f64, a temporary f64 plan
+    // for f32.  Plan-time launches stay out of the caller's launch record.
+    const std::vector<LaunchRec> saved = g_launch_log;
+    {
+        Plan<double>* p64 = nullptr;
+        std::unique_ptr<Plan<double>> tmp;
+        if constexpr (std::is_same<T, double>::value) {
+            p64 = pl->inner;
+        } else {
+            if (int32_t st = build_plan<double>(M, device, &p64)) { g_launch_log = saved; return st; }
+            tmp.reset(p64);
+        }
+        Io<double> io;
+        io.in_re = reinterpret_cast<const double*>(b); io.in_im = nullptr; io.out_re = reinterpret_cast<double*>(b); io.out_im = nullptr;
+        io.in_bstride = io.out_bstride = (long long)M;
+        io.in_il = io.out_il = 1;
+        int32_t st = run_c2c(*p64, io, 1, 1.0 / (double)M, p64->stream);
+        g_launch_log = saved;
+        if (st) return st;
+        CUDA_TRY(cudaStreamSynchronize(p64->stream));
+    }
+    if constexpr (std::is_same<T, double>::value) {
+        pl->bhat = b_owner.release();
+    } else {
+        CUDA_TRY(cudaMalloc(&pl->bhat, M * sizeof(cx<T>)));
+        chirp_narrow_kernel<T><<<(unsigned)std::min<size_t>((M + 255) / 256, 65536), 256>>>(b, pl->bhat, (long long)M);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaDeviceSynchronize());
+    }
+    CUDA_TRY(cudaMalloc(&pl->ws, M * sizeof(cx<T>)));                // room for one member; batched calls grow it
+    pl->ws_members = 1;
+    CUDA_TRY(cudaEventCreateWithFlags(&pl->ws_free, cudaEventDisableTiming));
+    pl->description = "n=" + std::to_string(n) + prec + " any: Bluestein M=2^" + std::to_string(lm) + " | inner: " + pl->inner->description;
+    *out = pl.release();
+    return PHASTFT_OK;
+}
+
+enum ChirpKind { CHIRP_PRE, CHIRP_MUL, CHIRP_POST };
+
+// One CHIRP-* kernel over `members` batch members, `per` threads each: a member-major grid of 256-thread blocks (as launch_real),
+// several launches when it would exceed 2^31 - 1 blocks.  Launch record: R = M, C = the members of that launch.
+template <typename T>
+int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_t members, cudaStream_t stream) {
+    const size_t bpm = (per + 255) / 256;
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    for (size_t done = 0; done < members; done += max_members) {
+        const size_t nb = std::min(members - done, max_members);
+        ChirpParams<T> q = cp;
+        const long long off = (long long)done * cp.bstride;
+        q.in_re += off; q.in_im += off; q.out_re += off; q.out_im += off;
+        q.ws += done << cp.log2m;
+        q.blocks_per_member = (unsigned)bpm;
+        const dim3 grid((unsigned)(nb * bpm));
+        if (kind == CHIRP_PRE) chirp_pre_kernel<T><<<grid, 256, 0, stream>>>(q);
+        else if (kind == CHIRP_MUL) chirp_mul_kernel<T><<<grid, 256, 0, stream>>>(q);
+        else chirp_post_kernel<T><<<grid, 256, 0, stream>>>(q);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({kind == CHIRP_PRE ? "CHIRP-PRE" : kind == CHIRP_MUL ? "CHIRP-MUL" : "CHIRP-POST", 1 << cp.log2m, 0, (int)nb, 256, 0,
+                     "plain", false});
+    }
+    return PHASTFT_OK;
+}
+
+// Grows the plan's workspace to `members` x M.  Caller holds pl->mu.  The new array is allocated before the old one is
+// released, so a failed allocation leaves the plan as it was.
+template <typename T>
+int32_t grow_any_workspace(const PlanAny<T>* pl, size_t members) {
+    if (pl->ws_members >= members) return PHASTFT_OK;
+    cx<T>* w = nullptr;
+    if (cudaMalloc(&w, (members << pl->log2m) * sizeof(cx<T>)) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return fail(PHASTFT_ERR_CUDA, "cudaMalloc of the plan's workspace for " + std::to_string(members) + " members failed");
+    }
+    CUDA_TRY(cudaDeviceSynchronize());   // every earlier user of the old workspace, on any stream, is done
+    cudaFree(pl->ws);
+    pl->ws = w; pl->ws_members = members;
+    return PHASTFT_OK;
+}
+
+// planar, in place, device pointers: the semantics of fft_dev for any N
+template <typename T>
+int32_t any_dev(const PlanAny<T>* pl, T* d_re, T* d_im, int direction, size_t batch, size_t bstride, cudaStream_t stream) {
+    if (!pl || !d_re || !d_im) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
+    if (direction != PHASTFT_FORWARD && direction != PHASTFT_REVERSE) return fail(PHASTFT_ERR_INVALID_ARG, "direction must be 1 or -1");
+    if (batch > 1 && bstride < pl->n) return fail(PHASTFT_ERR_INVALID_ARG, "batch_stride < N");
+    if (!pl->log2m) return fft_dev(pl->inner, d_re, d_im, direction, batch, bstride, stream);
+    if (batch == 0) return PHASTFT_OK;
+    DeviceGuard g(pl->device);
+    const size_t M = size_t(1) << pl->log2m;
+    std::lock_guard<std::mutex> lock(pl->mu);
+    // the workspace protocol of run_c2c: grown (synchronising) outside a capture only; a caller on another stream first waits for
+    // the previous user
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+    const bool capturing = cap != cudaStreamCaptureStatusNone;
+    if (pl->ws_members < batch) {
+        if (capturing)
+            return fail(PHASTFT_ERR_INVALID_ARG, "the plan's workspace is too small for this batch and the stream is being captured: "
+                                                 "call phastft_plan_any_*_reserve(batch) before capturing");
+        if (int32_t st = grow_any_workspace(pl, batch)) return st;
+    }
+    if (!capturing && pl->ws_used && pl->ws_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, pl->ws_free, 0));
+    // the reverse direction by the swap trick (fft_dev): re and im exchanged on the way in and out, 1/N folded into CHIRP-POST
+    const bool fwd = direction == PHASTFT_FORWARD;
+    ChirpParams<T> cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.in_re = cp.out_re = fwd ? d_re : d_im;
+    cp.in_im = cp.out_im = fwd ? d_im : d_re;
+    cp.ws = pl->ws; cp.chirp = pl->chirp; cp.bhat = pl->bhat;
+    cp.bstride = (long long)bstride; cp.n = (long long)pl->n; cp.log2m = pl->log2m;
+    cp.scale = fwd ? T(1) : T(1) / (T)pl->n;
+    constexpr size_t V = Cx16<T>::V;
+    Io<T> io;
+    io.in_re = reinterpret_cast<const T*>(pl->ws); io.in_im = nullptr;
+    io.out_re = reinterpret_cast<T*>(pl->ws); io.out_im = nullptr;
+    io.in_bstride = io.out_bstride = (long long)M;
+    io.in_il = io.out_il = 1;
+    if (int32_t st = launch_chirp(CHIRP_PRE, cp, M / V, batch, stream)) return st;
+    if (int32_t st = run_c2c(*pl->inner, io, batch, T(1), stream)) return st;
+    if (int32_t st = launch_chirp(CHIRP_MUL, cp, M / V, batch, stream)) return st;
+    if (int32_t st = run_c2c(*pl->inner, io, batch, T(1), stream)) return st;
+    if (int32_t st = launch_chirp(CHIRP_POST, cp, (pl->n + V - 1) / V, batch, stream)) return st;
+    if (!capturing) {
+        CUDA_TRY(cudaEventRecord(pl->ws_free, stream));
+        pl->ws_last_stream = stream;
+        pl->ws_used = true;
+    }
+    return PHASTFT_OK;
+}
+
+// Every allocation a call of `batch` would make: the inner plan's workspace and this plan's.
+template <typename T>
+int32_t any_reserve(const PlanAny<T>* pl, size_t batch) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (int32_t st = plan_reserve(pl->inner, batch)) return st;
+    if (!pl->log2m) return PHASTFT_OK;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->mu);
+    return grow_any_workspace(pl, batch);
+}
+
+// host slices: H2D, run, D2H, synchronous (fft_host for any N)
+template <typename T>
+int32_t any_host(const PlanAny<T>* pl, T* re, size_t len_re, T* im, size_t len_im, int direction) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (len_re != len_im) return fail(PHASTFT_ERR_LEN_MISMATCH);
+    if (len_re != pl->n) return fail(PHASTFT_ERR_PLAN_MISMATCH, "slice length " + std::to_string(len_re) + ", plan n = " + std::to_string(pl->n));
+    if (direction != PHASTFT_FORWARD && direction != PHASTFT_REVERSE) return fail(PHASTFT_ERR_INVALID_ARG, "direction must be 1 or -1");
+    if (!re || !im) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    if (!pl->log2m) return fft_host(pl->inner, re, len_re, im, len_im, direction);
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    {
+        std::lock_guard<std::mutex> lock(pl->mu);       // released before any_dev, which takes it
+        if (!pl->stage_re) CUDA_TRY(cudaMalloc(&pl->stage_re, pl->n * sizeof(T)));
+        if (!pl->stage_im) CUDA_TRY(cudaMalloc(&pl->stage_im, pl->n * sizeof(T)));
+    }
+    cudaStream_t s = pl->inner->stream;
+    const size_t bytes = pl->n * sizeof(T);
+    CUDA_TRY(cudaMemcpyAsync(pl->stage_re, re, bytes, cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(pl->stage_im, im, bytes, cudaMemcpyHostToDevice, s));
+    if (int32_t st = any_dev(pl, pl->stage_re, pl->stage_im, direction, 1, pl->n, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(re, pl->stage_re, bytes, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(im, pl->stage_im, bytes, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -2247,6 +2546,8 @@ int32_t oneshot_r2c_plan(OneShotCache<PlanR2c<T>>& c, size_t n, int device, Plan
 #define AS_CPLAN(T, p) reinterpret_cast<const Plan<T>*>(p)
 #define AS_R2C(T, p) reinterpret_cast<PlanR2c<T>*>(p)
 #define AS_CR2C(T, p) reinterpret_cast<const PlanR2c<T>*>(p)
+#define AS_ANY(T, p) reinterpret_cast<PlanAny<T>*>(p)
+#define AS_CANY(T, p) reinterpret_cast<const PlanAny<T>*>(p)
 
 extern "C" {
 
@@ -2460,6 +2761,31 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                     T* sim, void* s) {                                                                  \
         launches_reset();                                                                                               \
         return c2r_dev<T>(AS_CR2C(T, p), ire, iim, out, sre, sim, (cudaStream_t)s);                                     \
+    }                                                                                                                   \
+    int32_t phastft_plan_any_##SFX##_create(size_t n, int device, phastft_plan_any_##SFX** out) {                       \
+        PlanAny<T>* pl = nullptr;                                                                                       \
+        int32_t st = build_plan_any<T>(n, device, &pl);                                                                 \
+        if (out) *out = reinterpret_cast<phastft_plan_any_##SFX*>(pl);                                                  \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    void phastft_plan_any_##SFX##_destroy(phastft_plan_any_##SFX* p) { delete AS_ANY(T, p); }                           \
+    size_t phastft_plan_any_##SFX##_size(const phastft_plan_any_##SFX* p) { return p ? AS_CANY(T, p)->n : 0; }          \
+    const char* phastft_plan_any_##SFX##_describe(const phastft_plan_any_##SFX* p) {                                    \
+        return p ? AS_CANY(T, p)->description.c_str() : "";                                                             \
+    }                                                                                                                   \
+    int32_t phastft_plan_any_##SFX##_reserve(const phastft_plan_any_##SFX* p, size_t batch) {                           \
+        return any_reserve<T>(AS_CANY(T, p), batch);                                                                    \
+    }                                                                                                                   \
+    int32_t phastft_fft_any_##SFX##_dev(const phastft_plan_any_##SFX* p, T* re, T* im, int dir, size_t batch,          \
+                                        size_t bstride, void* s) {                                                      \
+        launches_reset();                                                                                               \
+        return any_dev<T>(AS_CANY(T, p), re, im, dir, batch, bstride, (cudaStream_t)s);                                 \
+    }                                                                                                                   \
+    int32_t phastft_fft_any_##SFX##_host(const phastft_plan_any_##SFX* p, T* re, size_t lre, T* im, size_t lim,        \
+                                         int dir) {                                                                     \
+        launches_reset();                                                                                               \
+        return any_host<T>(AS_CANY(T, p), re, lre, im, lim, dir);                                                       \
     }
 
 DEFINE_DIT_API(double, f64)

@@ -20,7 +20,7 @@ pub mod options;
 pub mod planner;
 
 use options::Options;
-use planner::{Direction, PlannerDit32, PlannerDit64, PlannerR2c32, PlannerR2c64};
+use planner::{Direction, PlannerAny32, PlannerAny64, PlannerDit32, PlannerDit64, PlannerR2c32, PlannerR2c64};
 
 /// Reference panic texts by status code (include/phastft_status.h).
 #[track_caller]
@@ -216,6 +216,31 @@ pub unsafe fn c2r_fft_f32_device(d_in_re: *const f32, d_in_im: *const f32, d_out
                                  d_scratch_re: *mut f32, d_scratch_im: *mut f32, stream: *mut std::os::raw::c_void) {
     check(ffi::phastft_c2r_f32_dev(planner.raw, d_in_re, d_in_im, d_output, d_scratch_re, d_scratch_im, stream));
 }
+
+// ------------------------------------------------------------------------------------------------
+// Additive: complex FFTs of any length (the reference accepts powers of two only)
+// ------------------------------------------------------------------------------------------------
+macro_rules! impl_any {
+    ($with_planner:ident, $device_batch:ident, $t:ty, $planner:ident, $ffi_host:ident, $ffi_dev:ident) => {
+        /// In place on planar host slices of `planner.num_points()` points, any length; forward unscaled, reverse scaled by
+        /// 1/N.  Panics on a length mismatch or a planner built for another size.
+        pub fn $with_planner(reals: &mut [$t], imags: &mut [$t], direction: Direction, planner: &$planner) {
+            check(unsafe { ffi::$ffi_host(planner.raw, reals.as_mut_ptr(), reals.len(), imags.as_mut_ptr(), imags.len(), direction as i32) });
+        }
+        /// Device-resident planar data, `batch` transforms at `b * batch_stride` (batch_stride >= N), stream-ordered on
+        /// `stream`; allocates only when the plan's workspace must grow (see `reserve`).
+        ///
+        /// # Safety
+        /// `d_reals` / `d_imags` must be device pointers valid for `(batch - 1) * batch_stride + n` elements on the
+        /// planner's device, and must not be used by other work on other streams until this call's work has completed.
+        pub unsafe fn $device_batch(d_reals: *mut $t, d_imags: *mut $t, direction: Direction, planner: &$planner, batch: usize,
+                                    batch_stride: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$ffi_dev(planner.raw, d_reals, d_imags, direction as i32, batch, batch_stride, stream));
+        }
+    };
+}
+impl_any!(fft_64_any_with_planner, fft_64_any_device_batch, f64, PlannerAny64, phastft_fft_any_f64_host, phastft_fft_any_f64_dev);
+impl_any!(fft_32_any_with_planner, fft_32_any_device_batch, f32, PlannerAny32, phastft_fft_any_f32_host, phastft_fft_any_f32_dev);
 
 // ------------------------------------------------------------------------------------------------
 // r2c / c2r  (algorithms/r2c.rs:521-895)

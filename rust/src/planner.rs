@@ -97,3 +97,44 @@ impl_planner_r2c!(PlannerR2c64, ffi::phastft_plan_r2c_f64, phastft_plan_r2c_f64_
                   phastft_plan_r2c_f64_reserve);
 impl_planner_r2c!(PlannerR2c32, ffi::phastft_plan_r2c_f32, phastft_plan_r2c_f32_create, phastft_plan_r2c_f32_destroy,
                   phastft_plan_r2c_f32_reserve);
+
+macro_rules! impl_planner_any {
+    ($name:ident, $raw:ty, $create:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
+        /// Additive (the reference accepts powers of two only): a complex FFT of any length.  A power of two runs the c2c plan
+        /// as it is; any other length up to 2^29 - 1 runs Bluestein's algorithm over a power-of-two plan.
+        pub struct $name {
+            pub(crate) raw: *mut $raw,
+        }
+        unsafe impl Send for $name {}
+        unsafe impl Sync for $name {}
+        impl $name {
+            /// Panics for `num_points == 0` or a length above 2^29 - 1 that is not a power of two.
+            pub fn new(num_points: usize) -> Self {
+                let mut raw = std::ptr::null_mut();
+                check(unsafe { ffi::$create(num_points, device(), &mut raw) });
+                Self { raw }
+            }
+            /// Number of points the planner was built for.
+            pub fn num_points(&self) -> usize {
+                unsafe { ffi::$size(self.raw) }
+            }
+            /// `"n=1000 f64 any: Bluestein M=2^11 | inner: ..."` or `"n=2^20 f64 any: power of two | inner: ..."`.
+            pub fn describe(&self) -> String {
+                unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
+            }
+            /// Makes every allocation a call of `batch` transforms would make, so such calls can be captured in a CUDA graph.
+            pub fn reserve(&self, batch: usize) {
+                check(unsafe { ffi::$reserve(self.raw, batch) });
+            }
+        }
+        impl Drop for $name {
+            fn drop(&mut self) {
+                unsafe { ffi::$destroy(self.raw) }
+            }
+        }
+    };
+}
+impl_planner_any!(PlannerAny64, ffi::phastft_plan_any_f64, phastft_plan_any_f64_create, phastft_plan_any_f64_destroy,
+                  phastft_plan_any_f64_size, phastft_plan_any_f64_describe, phastft_plan_any_f64_reserve);
+impl_planner_any!(PlannerAny32, ffi::phastft_plan_any_f32, phastft_plan_any_f32_create, phastft_plan_any_f32_destroy,
+                  phastft_plan_any_f32_size, phastft_plan_any_f32_describe, phastft_plan_any_f32_reserve);
