@@ -70,7 +70,7 @@ template <> struct Api<double> {
     static int32_t r2c_host(const R2c* p, const double* in, std::size_t li, double* ore, std::size_t lre, double* oim, std::size_t lim) { return phastft_r2c_f64_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const double* ire, std::size_t lre, const double* iim, std::size_t lim, double* out, std::size_t lo, double* sre, std::size_t lsr, double* sim, std::size_t lsi) { return phastft_c2r_f64_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
     using Any = phastft_plan_any_f64;
-    static int32_t any_create(std::size_t n, int dev, Any** o) { return phastft_plan_any_f64_create(n, dev, o); }
+    static int32_t any_create(std::size_t n, int dev, int algo, Any** o) { return phastft_plan_any_f64_create_with(n, dev, algo, o); }
     static void any_destroy(Any* p) { phastft_plan_any_f64_destroy(p); }
     static std::size_t any_size(const Any* p) { return phastft_plan_any_f64_size(p); }
     static const char* any_describe(const Any* p) { return phastft_plan_any_f64_describe(p); }
@@ -109,7 +109,7 @@ template <> struct Api<float> {
     static int32_t r2c_host(const R2c* p, const float* in, std::size_t li, float* ore, std::size_t lre, float* oim, std::size_t lim) { return phastft_r2c_f32_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_host(const R2c* p, const float* ire, std::size_t lre, const float* iim, std::size_t lim, float* out, std::size_t lo, float* sre, std::size_t lsr, float* sim, std::size_t lsi) { return phastft_c2r_f32_host(p, ire, lre, iim, lim, out, lo, sre, lsr, sim, lsi); }
     using Any = phastft_plan_any_f32;
-    static int32_t any_create(std::size_t n, int dev, Any** o) { return phastft_plan_any_f32_create(n, dev, o); }
+    static int32_t any_create(std::size_t n, int dev, int algo, Any** o) { return phastft_plan_any_f32_create_with(n, dev, algo, o); }
     static void any_destroy(Any* p) { phastft_plan_any_f32_destroy(p); }
     static std::size_t any_size(const Any* p) { return phastft_plan_any_f32_size(p); }
     static const char* any_describe(const Any* p) { return phastft_plan_any_f32_describe(p); }
@@ -178,17 +178,24 @@ class PlannerR2c {
     typename Api<T>::R2c* raw_ = nullptr;
 };
 
-/// additive: a complex FFT of any length (a power of two runs the c2c plan; any other length up to 2^29 - 1, Bluestein's algorithm)
+/// How a length that is not a power of two is transformed (PHASTFT_ANY_*).  Auto takes Mixed for every eligible length
+/// (2^a 3^b 5^c 7^d below 2^30 whose odd part fits one or two odd passes) and Bluestein otherwise, from the factorisation alone.
+enum class AnyAlgo : int { Bluestein = PHASTFT_ANY_BLUESTEIN, Mixed = PHASTFT_ANY_MIXED, Auto = PHASTFT_ANY_AUTO };
+
+/// additive: a complex FFT of any length (a power of two runs the c2c plan; any other length up to 2^29 - 1 Bluestein's
+/// algorithm, or with AnyAlgo::Mixed / AnyAlgo::Auto the mixed-radix path for smooth lengths below 2^30)
 template <typename T>
 class PlannerAny {
   public:
-    explicit PlannerAny(std::size_t num_points, int device = 0) { check(Api<T>::any_create(num_points, device, &raw_)); }
+    explicit PlannerAny(std::size_t num_points, int device = 0, AnyAlgo algo = AnyAlgo::Bluestein) {
+        check(Api<T>::any_create(num_points, device, static_cast<int>(algo), &raw_));
+    }
     ~PlannerAny() { if (raw_) Api<T>::any_destroy(raw_); }
     PlannerAny(PlannerAny&& o) noexcept : raw_(o.raw_) { o.raw_ = nullptr; }
     PlannerAny(const PlannerAny&) = delete;
     PlannerAny& operator=(const PlannerAny&) = delete;
     std::size_t num_points() const { return Api<T>::any_size(raw_); }
-    /// "power of two" or "Bluestein M=2^m", then the inner plan's description
+    /// "power of two", "Bluestein M=2^m" or "mixed 2^a x Q_a[ x Q_b]", then the inner plan's description
     std::string describe() const { return Api<T>::any_describe(raw_); }
     /// make every allocation a call of `batch` transforms would make now
     void reserve(std::size_t batch) const { check(Api<T>::any_reserve(raw_, batch)); }
@@ -246,6 +253,7 @@ using PlannerDit64 = detail::PlannerDit<double>;
 using PlannerDit32 = detail::PlannerDit<float>;
 using PlannerR2c64 = detail::PlannerR2c<double>;
 using PlannerR2c32 = detail::PlannerR2c<float>;
+using AnyAlgo = detail::AnyAlgo;
 using PlannerAny64 = detail::PlannerAny<double>;
 using PlannerAny32 = detail::PlannerAny<float>;
 using PlannerR2cAny64 = detail::PlannerR2cAny<double>;

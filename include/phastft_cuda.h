@@ -47,7 +47,9 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * passes), ROW (one CTA per transform), CLUSTER (both passes in one cluster launch: R=<R1>x<R2>, K=<CTAs per cluster>),
  * PIPE (both passes in one pipelined launch: R=<R1>x<R2>), R2C-UNTANGLE / C2R-PRE (the real transforms' elementwise
  * kernels), CHIRP-PRE / CHIRP-MUL / CHIRP-POST (the any-length transform's elementwise kernels: R=<M>, C=<members>), CHIRP-PRE-R2C /
- * CHIRP-POST-R2C / CHIRP-PRE-C2R / CHIRP-POST-C2R (the same around the real any-length transforms); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * CHIRP-POST-R2C / CHIRP-PRE-C2R / CHIRP-POST-C2R (the same around the real any-length transforms), SMOOTH-PRE (the mixed-radix
+ * path's de-interleave: R=<P>, C=<workspace members>) and ODD (its radix-3/5/7 passes: R=<rows>, C=<columns per CTA>, mode reg
+ * for the register kernel or tile for the shared-memory one); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
@@ -283,7 +285,28 @@ PHASTFT_API size_t phastft_plan_any_f32_size(const phastft_plan_any_f32* plan);
 /* "n=1000 f64 any: Bluestein M=2^11 | inner: n=2^11 f64: ..." or "n=2^20 f64 any: power of two | inner: n=2^20 f64: ..." */
 PHASTFT_API const char* phastft_plan_any_f64_describe(const phastft_plan_any_f64* plan);
 PHASTFT_API const char* phastft_plan_any_f32_describe(const phastft_plan_any_f32* plan);
-/* Makes every allocation a call of `batch` transforms would make now: the inner plan's workspace and this plan's batch * M.
+/* The algorithm of a length that is not a power of two (a power of two takes the c2c plan under every value):
+ *   PHASTFT_ANY_BLUESTEIN  Bluestein, as phastft_plan_any_*_create builds.
+ *   PHASTFT_ANY_MIXED      the mixed-radix path for n = P * Q < 2^30, P = 2^a, Q = 3^b 5^c 7^d > 1: SMOOTH-PRE de-interleaves the
+ *                          input by Q into a workspace of n complex values, the P-point plan transforms its Q * batch members,
+ *                          and one ODD pass (Q <= 729) or two (Q = Q_a * Q_b, both <= 729, the most balanced split) run the
+ *                          Q-point DFTs with the W_n twiddles and store in natural order.  No padding: about 8n values through
+ *                          device memory where Bluestein moves 40n to 50n.  A length with another prime factor, or whose odd part
+ *                          has no such split, returns PHASTFT_ERR_INVALID_ARG (the detail names the factor) before the device is
+ *                          touched.  Smooth lengths between 2^29 and 2^30 run on this path only.
+ *   PHASTFT_ANY_AUTO       mixed when n is eligible, Bluestein otherwise: decided from the factorisation of n alone.  The value
+ *                          to pass unless one algorithm is wanted.
+ * describe(): "n=1000000 f64 any: mixed 2^6 x 125 x 125 | inner: n=2^6 f64: ..." ("mixed 2^20 x 3" with one odd pass). */
+#define PHASTFT_ANY_BLUESTEIN 0
+#define PHASTFT_ANY_MIXED 1
+#define PHASTFT_ANY_AUTO 2
+PHASTFT_API int32_t phastft_plan_any_f64_create_with(size_t n, int device, int algo, phastft_plan_any_f64** out);
+PHASTFT_API int32_t phastft_plan_any_f32_create_with(size_t n, int device, int algo, phastft_plan_any_f32** out);
+/* Host-only: the split n = p * q_a * q_b of the mixed-radix path (q_b = 1: one odd pass; the same for both precisions), or
+ * PHASTFT_ERR_INVALID_ARG with the reason when n is not eligible. */
+PHASTFT_API int32_t phastft_any_mixed_factorization(size_t n, size_t* p, int* q_a, int* q_b);
+/* Makes every allocation a call of `batch` transforms would make now: the inner plan's workspace and this plan's batch * M
+ * (mixed: batch * n).
  * A call that would grow either while its stream is being captured into a CUDA graph returns PHASTFT_ERR_INVALID_ARG. */
 PHASTFT_API int32_t phastft_plan_any_f64_reserve(const phastft_plan_any_f64* plan, size_t batch);
 PHASTFT_API int32_t phastft_plan_any_f32_reserve(const phastft_plan_any_f32* plan, size_t batch);

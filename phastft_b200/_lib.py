@@ -107,6 +107,7 @@ SIGNATURES = {
     "phastft_r2c_{s}_batch_dev": ([_vp, _vp, _sz, _vp, _vp, _sz, _sz, _vp], _i32),
     "phastft_c2r_{s}_batch_dev": ([_vp, _vp, _vp, _sz, _vp, _sz, _vp, _vp, _sz, _vp], _i32),
     "phastft_plan_any_{s}_create": ([_sz, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_any_{s}_create_with": ([_sz, _ci, _ci, C.POINTER(_vp)], _i32),
     "phastft_plan_any_{s}_destroy": ([_vp], None),
     "phastft_plan_any_{s}_size": ([_vp], _sz),
     "phastft_plan_any_{s}_describe": ([_vp], C.c_char_p),
@@ -147,6 +148,18 @@ def plan_factorization(n: int, precision_bits: int = 64):
     return [f[i] for i in range(k.value)]
 
 
+lib.phastft_any_mixed_factorization.argtypes = [_sz, C.POINTER(_sz), C.POINTER(_ci), C.POINTER(_ci)]
+lib.phastft_any_mixed_factorization.restype = _i32
+
+
+def any_mixed_factorization(n: int):
+    """Host-only: (P, Q_a, Q_b) with n = P * Q_a * Q_b as the mixed-radix path splits it (Q_b = 1: one odd pass); raises
+    PhastFTPanic(13) naming the reason when n is not eligible."""
+    p, qa, qb = _sz(0), _ci(0), _ci(0)
+    check(lib.phastft_any_mixed_factorization(int(n), C.byref(p), C.byref(qa), C.byref(qb)))
+    return p.value, qa.value, qb.value
+
+
 lib.phastft_plan_tune_candidates.argtypes = [_sz, _ci, C.POINTER(_ci), C.POINTER(_ci), _ci, C.POINTER(_ci)]
 lib.phastft_plan_tune_candidates.restype = _i32
 
@@ -166,7 +179,7 @@ def plan_tune_candidates(n: int, precision_bits: int = 64):
 
 
 GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization",
-                  "phastft_plan_tune_candidates", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
+                  "phastft_plan_tune_candidates", "phastft_any_mixed_factorization", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
                   "phastft_device_count", "phastft_options_default", "phastft_options_guess"]
 
 for _name, (_args, _res) in SIGNATURES.items():

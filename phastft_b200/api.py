@@ -39,7 +39,7 @@ __all__ = [
     "c2r_fft_f32_with_planner_and_scratch",
     "fft_dit_batch", "fft_dit_batch_sharded", "host_register", "host_unregister",
     "r2c_batch", "c2r_batch",
-    "PlannerAny64", "PlannerAny32", "fft_64_any_with_planner", "fft_32_any_with_planner", "fft_any_batch",
+    "AnyAlgo", "PlannerAny64", "PlannerAny32", "fft_64_any_with_planner", "fft_32_any_with_planner", "fft_any_batch",
     "PlannerR2cAny64", "PlannerR2cAny32", "r2c_fft_f64_any_with_planner", "r2c_fft_f32_any_with_planner",
     "c2r_fft_f64_any_with_planner", "c2r_fft_f32_any_with_planner", "r2c_any_batch", "c2r_any_batch",
 ]
@@ -228,25 +228,40 @@ class PlannerR2c32(_PlannerR2c):
     _sfx, _dtype = "f32", np.float32
 
 
+class AnyAlgo(enum.IntEnum):
+    """How a length that is not a power of two is transformed (include/phastft_cuda.h, PHASTFT_ANY_*).  Auto picks Mixed for
+    every eligible length (2^a 3^b 5^c 7^d below 2^30 whose odd part fits one or two odd passes) and Bluestein otherwise, from
+    the factorisation of the length alone: pass it unless one algorithm is wanted."""
+    Bluestein = 0
+    Mixed = 1
+    Auto = 2
+
+
 class _PlannerAny:
     _sfx = ""
     _dtype = None
 
-    def __init__(self, num_points: int, device: int = 0):
+    def __init__(self, num_points: int, device: int = 0, algo: AnyAlgo = AnyAlgo.Bluestein):
         """A complex FFT of any length num_points >= 1 (the reference accepts powers of two only): a power of two runs the
-        c2c plan as it is, any other length up to 2^29 - 1 Bluestein's algorithm over a power-of-two plan.  Other lengths
-        raise PhastFTPanic(13) before the device is touched."""
+        c2c plan as it is, any other length up to 2^29 - 1 Bluestein's algorithm over a power-of-two plan, or with
+        AnyAlgo.Mixed / AnyAlgo.Auto the mixed-radix path for smooth lengths below 2^30.  Other lengths (and AnyAlgo.Mixed on
+        a length that is not eligible) raise PhastFTPanic(13) before the device is touched."""
         self._h = C.c_void_p()
         self.device = int(device)
-        check(fn("phastft_plan_any_{s}_create", self._sfx)(int(num_points), self.device, C.byref(self._h)))
+        check(fn("phastft_plan_any_{s}_create_with", self._sfx)(int(num_points), self.device, int(algo), C.byref(self._h)))
         self.num_points = int(num_points)
 
     @classmethod
     def new(cls, num_points: int, device: int = 0):
         return cls(num_points, device)
 
+    @classmethod
+    def with_algo(cls, num_points: int, algo: AnyAlgo, device: int = 0):
+        return cls(num_points, device, algo)
+
     def describe(self) -> str:
-        """"power of two" or "Bluestein M=2^m" (the convolution length), then the inner plan's describe()."""
+        """"power of two", "Bluestein M=2^m" (the convolution length) or "mixed 2^a x Q_a[ x Q_b]", then the inner plan's
+        describe()."""
         return fn("phastft_plan_any_{s}_describe", self._sfx)(self._h).decode()
 
     def reserve(self, batch: int) -> None:

@@ -187,6 +187,71 @@ template <typename T> struct Dft<T, 32> {
 };
 
 // ---------------------------------------------------------------------------------------------
+// Forward DFTs of length 3/5/7 (the odd passes of the mixed-radix path), natural order in and out.  With a_j = x_j + x_(p-j)
+// and b_j = x_j - x_(p-j):  X_k = A_k - i B_k and X_(p-k) = A_k + i B_k,  A_k = x_0 + sum_j cos(2 pi jk/p) a_j,
+// B_k = sum_j sin(2 pi jk/p) b_j: real constants times complex values, all in FMA form.
+// ---------------------------------------------------------------------------------------------
+// (X_k, X_(p-k)) from A and B
+template <typename T>
+__device__ __forceinline__ void odd_pair(T ar, T ai, T br, T bi, T& kr, T& ki, T& mr, T& mi) {
+    kr = ar + bi; ki = ai - br;
+    mr = ar - bi; mi = ai + br;
+}
+
+template <typename T> struct Dft<T, 3> {
+    static __device__ __forceinline__ void run(T (&r)[3], T (&i)[3]) {
+        const T s = T(0.8660254037844386467637231707529361834714);  // sin(2pi/3)
+        const T ar = r[1] + r[2], ai = i[1] + i[2];
+        const T br = s * (r[1] - r[2]), bi = s * (i[1] - i[2]);
+        const T mr = fma_t(T(-0.5), ar, r[0]), mi = fma_t(T(-0.5), ai, i[0]);
+        r[0] += ar; i[0] += ai;
+        odd_pair(mr, mi, br, bi, r[1], i[1], r[2], i[2]);
+    }
+};
+
+template <typename T> struct Dft<T, 5> {
+    static __device__ __forceinline__ void run(T (&r)[5], T (&i)[5]) {
+        const T c1 = T(0.3090169943749474241022934171828190588602);   // cos(2pi/5)
+        const T c2 = T(-0.8090169943749474241022934171828190588602);  // cos(4pi/5)
+        const T s1 = T(0.9510565162951535721164393333793821434057);   // sin(2pi/5)
+        const T s2 = T(0.5877852522924731291687059546390727685977);   // sin(4pi/5)
+        const T a1r = r[1] + r[4], a1i = i[1] + i[4], b1r = r[1] - r[4], b1i = i[1] - i[4];
+        const T a2r = r[2] + r[3], a2i = i[2] + i[3], b2r = r[2] - r[3], b2i = i[2] - i[3];
+        const T A1r = fma_t(c2, a2r, fma_t(c1, a1r, r[0])), A1i = fma_t(c2, a2i, fma_t(c1, a1i, i[0]));
+        const T A2r = fma_t(c1, a2r, fma_t(c2, a1r, r[0])), A2i = fma_t(c1, a2i, fma_t(c2, a1i, i[0]));
+        const T B1r = fma_t(s2, b2r, s1 * b1r), B1i = fma_t(s2, b2i, s1 * b1i);
+        const T B2r = fma_t(-s1, b2r, s2 * b1r), B2i = fma_t(-s1, b2i, s2 * b1i);
+        r[0] += a1r + a2r; i[0] += a1i + a2i;
+        odd_pair(A1r, A1i, B1r, B1i, r[1], i[1], r[4], i[4]);
+        odd_pair(A2r, A2i, B2r, B2i, r[2], i[2], r[3], i[3]);
+    }
+};
+
+template <typename T> struct Dft<T, 7> {
+    static __device__ __forceinline__ void run(T (&r)[7], T (&i)[7]) {
+        const T c1 = T(0.6234898018587335305250048840042398106323);   // cos(2pi/7)
+        const T c2 = T(-0.2225209339563144042889025644967947594664);  // cos(4pi/7)
+        const T c3 = T(-0.9009688679024191262361023195074450511659);  // cos(6pi/7)
+        const T s1 = T(0.7818314824680298087084445266740577502323);   // sin(2pi/7)
+        const T s2 = T(0.9749279121818236070181316829939312172328);   // sin(4pi/7)
+        const T s3 = T(0.4338837391175581204757683328483587546100);   // sin(6pi/7)
+        const T a1r = r[1] + r[6], a1i = i[1] + i[6], b1r = r[1] - r[6], b1i = i[1] - i[6];
+        const T a2r = r[2] + r[5], a2i = i[2] + i[5], b2r = r[2] - r[5], b2i = i[2] - i[5];
+        const T a3r = r[3] + r[4], a3i = i[3] + i[4], b3r = r[3] - r[4], b3i = i[3] - i[4];
+        const T A1r = fma_t(c3, a3r, fma_t(c2, a2r, fma_t(c1, a1r, r[0]))), A1i = fma_t(c3, a3i, fma_t(c2, a2i, fma_t(c1, a1i, i[0])));
+        const T A2r = fma_t(c1, a3r, fma_t(c3, a2r, fma_t(c2, a1r, r[0]))), A2i = fma_t(c1, a3i, fma_t(c3, a2i, fma_t(c2, a1i, i[0])));
+        const T A3r = fma_t(c2, a3r, fma_t(c1, a2r, fma_t(c3, a1r, r[0]))), A3i = fma_t(c2, a3i, fma_t(c1, a2i, fma_t(c3, a1i, i[0])));
+        const T B1r = fma_t(s3, b3r, fma_t(s2, b2r, s1 * b1r)), B1i = fma_t(s3, b3i, fma_t(s2, b2i, s1 * b1i));
+        const T B2r = fma_t(-s1, b3r, fma_t(-s3, b2r, s2 * b1r)), B2i = fma_t(-s1, b3i, fma_t(-s3, b2i, s2 * b1i));
+        const T B3r = fma_t(s2, b3r, fma_t(-s1, b2r, s3 * b1r)), B3i = fma_t(s2, b3i, fma_t(-s1, b2i, s3 * b1i));
+        r[0] += a1r + a2r + a3r; i[0] += a1i + a2i + a3i;
+        odd_pair(A1r, A1i, B1r, B1i, r[1], i[1], r[6], i[6]);
+        odd_pair(A2r, A2i, B2r, B2i, r[2], i[2], r[5], i[5]);
+        odd_pair(A3r, A3i, B3r, B3i, r[3], i[3], r[4], i[4]);
+    }
+};
+
+// ---------------------------------------------------------------------------------------------
 // Complex-array interface of the DFTs: DftC<T, RAD>::run(x[RAD]) and ctwid(a, w) = a * w.
 // Both precisions unpack into the split re/im arrays above (the reference's fma(2, lo, -out0) butterfly,
 // kernels/dit.rs:181-183).  The float twiddle product rounds a.y*w.x (not a.x*w.y) before its imaginary FMA; the

@@ -1139,4 +1139,214 @@ __global__ void __launch_bounds__(256) chirp_narrow_kernel(const double2* __rest
         out[i] = make_cx<T>((T)in[i].x, (T)in[i].y);
 }
 
+// ---------------------------------------------------------------------------------------------
+// Mixed radix (N = P * Q, P = 2^a, Q = 3^b 5^c 7^d > 1; phastft_fft_any_* with PHASTFT_ANY_MIXED): with n = n_o + Q n_2 and
+// k = k_2 + P k_o,  X[k_2 + P k_o] = sum_(n_o) W_Q^(n_o k_o) W_N^(n_o k_2) Y_(n_o)[k_2],  Y_(n_o) = DFT_P(x[n_o + Q n_2]).
+//   SMOOTH-PRE  planar x -> workspace member n_o (P interleaved points), a tiled transpose by Q
+//   the P-point plan on Q * batch interleaved members in place
+//   ODD         Q <= ODD_MAX_ROWS: one pass, W_N^(n_o k_2) on load, the Q-point DFT down the member axis, planar store.
+//               Otherwise Q = Q_a Q_b, n_o = n_a Q_b + n_b, k_o = k_a + Q_a k_b: pass A (W_N^(n_o k_2) on load, n_a -> k_a in place
+//               in the workspace, rows Q_b P apart), pass B (W_Q^(n_b k_a) on load, n_b -> k_b, planar store of row k_a + Q_a k_b).
+// Every pass is "R rows, N / R columns per member": column c of member m reads rows r at in0 + r * in_rs, multiplies by
+// W_N^(e0 + r * de) and writes row k at c + k * out_rs.
+// ---------------------------------------------------------------------------------------------
+enum OddRole { ODD_SINGLE, ODD_A, ODD_B };
+constexpr int ODD_MAX_STAGES = 6;      // 3^6 = 729
+constexpr int ODD_MAX_ROWS = 729;      // the largest tile: 729 rows x 128 bytes = 91 KiB, two CTAs per SM
+constexpr int ODD_NT = 256;
+
+template <typename T>
+struct OddParams {
+    const cx<T>* ws;               // batch x N interleaved: every pass reads it, pass A writes it
+    cx<T>* ws_out;
+    T* out_re;                     // the last pass: the caller's planar arrays (re / im swapped for the reverse direction)
+    T* out_im;
+    const cx<T>* wn_hi;            // W_N^(j << lo_bits)
+    const cx<T>* wn_lo;            // W_N^j, j < 2^lo_bits
+    const cx<T>* wr;               // W_R^j, j < R: the twiddles between the stages of this pass
+    const unsigned short* perm;    // tile kernel: where stage 1 puts the butterfly of row r < R / rad[0] (digit reversal)
+    long long n, p, cols, total;   // N, P, columns per member (N / R), batch * cols
+    long long in_rs, out_rs;       // elements between rows
+    long long bstride;             // elements between members of the caller's arrays
+    int role, r, qb, lo_bits;
+    int nstages, rad[ODD_MAX_STAGES];
+    int cw;                        // tile kernel: columns per CTA
+    T scale;                       // the last pass: 1 forward, 1/N reverse
+};
+
+// One column of a pass: where its rows are, its twiddle exponents and where its output rows go.
+template <typename T>
+struct OddCol {
+    const cx<T>* in;
+    cx<T>* out_c;
+    T* out_re;
+    T* out_im;
+    unsigned long long e0, de;
+    __device__ __forceinline__ OddCol(const OddParams<T>& p, long long g) {
+        const long long m = g / p.cols, c = g - m * p.cols;
+        const long long hi = p.role == ODD_SINGLE ? 0 : c / p.p, lo = c - hi * p.p;
+        in = p.ws + m * p.n + (p.role == ODD_B ? hi * p.qb * p.p + lo : c);
+        e0 = p.role == ODD_A ? hi * lo : 0;
+        de = p.role == ODD_SINGLE ? lo : p.role == ODD_A ? p.qb * lo : hi * p.p;
+        out_c = p.ws_out + m * p.n + c;
+        out_re = p.out_re + m * p.bstride + c;
+        out_im = p.out_im + m * p.bstride + c;
+    }
+    // row r, times W_N^(e0 + r de)
+    __device__ __forceinline__ cx<T> load(const OddParams<T>& p, int r) const {
+        const cx<T> v = in[r * p.in_rs];
+        const unsigned long long e = e0 + r * de;
+        if (e == 0) return v;
+        const cx<T> w = cmul<T>(__ldg(p.wn_hi + (e >> p.lo_bits)), __ldg(p.wn_lo + (e & ((1ull << p.lo_bits) - 1))));
+        return ctwid<T>(v, w);
+    }
+    __device__ __forceinline__ void store(const OddParams<T>& p, int k, const cx<T>& v) const {
+        if (p.role == ODD_A) {
+            out_c[k * p.out_rs] = v;
+        } else {
+            out_re[k * p.out_rs] = v.x * p.scale;
+            out_im[k * p.out_rs] = v.y * p.scale;
+        }
+    }
+};
+
+// R = RA * RB rows (RB = 1: one register DFT) held by one thread: no shared memory, a block covers ODD_NT adjacent columns.
+template <typename T, int RA, int RB>
+__global__ void __launch_bounds__(ODD_NT) odd_reg_kernel(const __grid_constant__ OddParams<T> p) {
+    constexpr int R = RA * RB;
+    const long long g = (long long)blockIdx.x * ODD_NT + threadIdx.x;
+    if (g >= p.total) return;
+    const OddCol<T> col(p, g);
+    cx<T> x[R];
+#pragma unroll
+    for (int r = 0; r < R; ++r) x[r] = col.load(p, r);
+    if constexpr (RB == 1) {
+        DftC<T, RA>::run(x);
+#pragma unroll
+        for (int k = 0; k < R; ++k) col.store(p, k, x[k]);
+    } else {
+        // n = n_a RB + n_b, k = k_a + RA k_b: DFT_RA over n_a, W_R^(n_b k_a), DFT_RB over n_b
+#pragma unroll
+        for (int nb = 0; nb < RB; ++nb) {
+            cx<T> a[RA];
+#pragma unroll
+            for (int na = 0; na < RA; ++na) a[na] = x[na * RB + nb];
+            DftC<T, RA>::run(a);
+#pragma unroll
+            for (int ka = 0; ka < RA; ++ka) x[ka * RB + nb] = nb * ka ? ctwid<T>(a[ka], __ldg(p.wr + nb * ka)) : a[ka];
+        }
+#pragma unroll
+        for (int ka = 0; ka < RA; ++ka) {
+            cx<T> b[RB];
+#pragma unroll
+            for (int nb = 0; nb < RB; ++nb) b[nb] = x[ka * RB + nb];
+            DftC<T, RB>::run(b);
+#pragma unroll
+            for (int kb = 0; kb < RB; ++kb) col.store(p, ka + RA * kb, b[kb]);
+        }
+    }
+}
+
+// One stage of the tile kernel over the butterflies row0, row0 + step, ...: FIRST reads the column's rows from global memory
+// (digit-reversed placement in the tile), LAST stores the output rows; the stages between work in place in shared memory.
+enum OddStage { ODD_FIRST, ODD_MID, ODD_LAST };
+template <typename T, int RAD, int STAGE>
+__device__ __forceinline__ void odd_tile_stage(const OddParams<T>& p, const OddCol<T>& col, cx<T>* sm, int L, int row0, int step,
+                                               bool live) {
+    const int nb = p.r / RAD;
+    for (int b = row0; b < nb; b += step) {
+        cx<T> x[RAD];
+        int base;
+        if constexpr (STAGE == ODD_FIRST) {
+            base = p.perm[b] * RAD;
+#pragma unroll
+            for (int q = 0; q < RAD; ++q) x[q] = col.load(p, b + q * nb);
+        } else {
+            const int t = b % L;
+            base = (b / L) * L * RAD + t;
+            const int ts = t * (nb / L);                               // W_(L RAD)^(q t) = W_R^(q t R / (L RAD))
+#pragma unroll
+            for (int q = 0; q < RAD; ++q) {
+                const cx<T> v = sm[(base + q * L) * p.cw];
+                x[q] = q && t ? ctwid<T>(v, __ldg(p.wr + q * ts)) : v;
+            }
+        }
+        DftC<T, RAD>::run(x);
+        if constexpr (STAGE == ODD_LAST) {
+            if (live) {
+#pragma unroll
+                for (int q = 0; q < RAD; ++q) col.store(p, base + q * L, x[q]);
+            }
+        } else {
+#pragma unroll
+            for (int q = 0; q < RAD; ++q) sm[(base + q * L) * p.cw] = x[q];
+        }
+    }
+}
+template <typename T, int STAGE>
+__device__ __forceinline__ void odd_tile_stage_of(int rad, const OddParams<T>& p, const OddCol<T>& col, cx<T>* sm, int L, int row0,
+                                                  int step, bool live) {
+    if (rad == 3) odd_tile_stage<T, 3, STAGE>(p, col, sm, L, row0, step, live);
+    else if (rad == 5) odd_tile_stage<T, 5, STAGE>(p, col, sm, L, row0, step, live);
+    else odd_tile_stage<T, 7, STAGE>(p, col, sm, L, row0, step, live);
+}
+
+// R rows x cw adjacent columns in shared memory (cw * sizeof(cx<T>) >= 128 bytes, so the interleaved loads and the planar
+// stores both move in runs of 64 bytes or more), radix-3/5/7 stages between __syncthreads().  Thread t owns column t % cw
+// and every (ODD_NT / cw)-th butterfly of it.
+template <typename T>
+__global__ void __launch_bounds__(ODD_NT, 2) odd_tile_kernel(const __grid_constant__ OddParams<T> p) {
+    extern __shared__ __align__(16) unsigned char odd_smem[];
+    const int c = threadIdx.x % p.cw, row0 = threadIdx.x / p.cw, step = ODD_NT / p.cw;
+    cx<T>* sm = reinterpret_cast<cx<T>*>(odd_smem) + c;
+    const long long g = (long long)blockIdx.x * p.cw + c;
+    const bool live = g < p.total;
+    const OddCol<T> col(p, live ? g : p.total - 1);                    // a dead column computes its neighbour's and stores nothing
+    odd_tile_stage_of<T, ODD_FIRST>(p.rad[0], p, col, sm, 1, row0, step, live);
+    int L = p.rad[0];
+    for (int s = 1; s + 1 < p.nstages; ++s) {
+        __syncthreads();
+        odd_tile_stage_of<T, ODD_MID>(p.rad[s], p, col, sm, L, row0, step, live);
+        L *= p.rad[s];
+    }
+    __syncthreads();
+    odd_tile_stage_of<T, ODD_LAST>(p.rad[p.nstages - 1], p, col, sm, L, row0, step, live);
+}
+
+// SMOOTH-PRE: ws[m N + n_o P + n_2] = (re, im)[m bstride + n_o + Q n_2].  A block transposes a tile of tq values of n_o by
+// tp values of n_2 through shared memory: it reads runs of tq adjacent elements and writes runs of tp adjacent complex values
+// (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).
+constexpr int SMOOTH_TILE = 1024;
+template <typename T>
+struct SmoothParams {
+    const T* in_re;                // swapped for the reverse direction
+    const T* in_im;
+    cx<T>* ws;
+    long long n, p, q, bstride;
+    int tq, tp;
+    unsigned tiles_q, tiles_per_member;
+};
+template <typename T>
+__global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__ SmoothParams<T> p) {
+    __shared__ cx<T> sm[2 * SMOOTH_TILE];
+    const unsigned m = blockIdx.x / p.tiles_per_member, tile = blockIdx.x - m * p.tiles_per_member;
+    const long long o = (long long)(tile % p.tiles_q) * p.tq, a = (long long)(tile / p.tiles_q) * p.tp;
+    const T* re = p.in_re + (long long)m * p.bstride;
+    const T* im = p.in_im + (long long)m * p.bstride;
+    const int count = p.tq * p.tp, pitch = p.tp + 1;
+    for (int i = threadIdx.x; i < count; i += 256) {
+        const int j2 = i / p.tq, jo = i - j2 * p.tq;
+        if (o + jo < p.q) {
+            const long long src = o + jo + p.q * (a + j2);
+            sm[jo * pitch + j2] = make_cx<T>(re[src], im[src]);
+        }
+    }
+    __syncthreads();
+    cx<T>* ws = p.ws + (long long)m * p.n;
+    for (int i = threadIdx.x; i < count; i += 256) {
+        const int jo = i / p.tp, j2 = i - jo * p.tp;
+        if (o + jo < p.q) ws[(o + jo) * p.p + a + j2] = sm[jo * pitch + j2];
+    }
+}
+
 }  // namespace phast

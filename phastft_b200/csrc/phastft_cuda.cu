@@ -2275,6 +2275,67 @@ int32_t oneshot_r2c_plan(OneShotCache<PlanR2c<T>>& c, size_t n, int device, Plan
 // power-of-two plan.
 constexpr size_t ANY_MAX_N = (size_t(1) << 29) - 1;
 
+// The interleaved workspace of an any-length plan (Bluestein's batch x M, the mixed-radix path's batch x N) and its protocol,
+// the one of run_c2c: grown (synchronising) outside a stream capture only; a caller on another stream first waits for the
+// previous user.  `mu` also guards the owner's host staging.
+template <typename T>
+struct AnyWorkspace {
+    std::mutex mu;
+    cx<T>* ws = nullptr;
+    size_t elems = 0;
+    cudaEvent_t free_ev = nullptr;     // orders workspace reuse across streams (like Plan::ws_free)
+    cudaStream_t last_stream = nullptr;
+    bool used = false;
+    int32_t init(size_t e) {
+        CUDA_TRY(cudaMalloc(&ws, e * sizeof(cx<T>)));
+        elems = e;
+        CUDA_TRY(cudaEventCreateWithFlags(&free_ev, cudaEventDisableTiming));
+        return PHASTFT_OK;
+    }
+    void destroy() {
+        if (free_ev) cudaEventDestroy(free_ev);
+        if (ws) cudaFree(ws);
+    }
+    // Grows to `e` values (`members` batch members).  Caller holds mu.  The new array is allocated before the old one is
+    // released, so a failed allocation leaves the plan as it was.
+    int32_t grow(size_t e, size_t members) {
+        if (elems >= e) return PHASTFT_OK;
+        cx<T>* w = nullptr;
+        if (cudaMalloc(&w, e * sizeof(cx<T>)) != cudaSuccess) {
+            (void)cudaGetLastError();
+            return fail(PHASTFT_ERR_CUDA, "cudaMalloc of the plan's workspace for " + std::to_string(members) + " members failed");
+        }
+        CUDA_TRY(cudaDeviceSynchronize());   // every earlier user of the old workspace, on any stream, is done
+        cudaFree(ws);
+        ws = w; elems = e;
+        return PHASTFT_OK;
+    }
+    // Before a call's first launch (caller holds mu): room for `e` values, and the previous user on another stream is done.
+    // `reserve_fn` names the call that grows the workspace ahead of a capture.
+    int32_t acquire(size_t e, size_t members, cudaStream_t stream, const char* reserve_fn, bool& capturing) {
+        cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+        CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+        capturing = cap != cudaStreamCaptureStatusNone;
+        if (elems < e) {
+            if (capturing)
+                return fail(PHASTFT_ERR_INVALID_ARG, std::string("the plan's workspace is too small for this batch and the stream is being "
+                                                                 "captured: call ") + reserve_fn + "(batch) before capturing");
+            if (int32_t st = grow(e, members)) return st;
+        }
+        if (!capturing && used && last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, free_ev, 0));
+        return PHASTFT_OK;
+    }
+    // After a call's last launch.
+    int32_t release(cudaStream_t stream, bool capturing) {
+        if (!capturing) {
+            CUDA_TRY(cudaEventRecord(free_ev, stream));
+            last_stream = stream;
+            used = true;
+        }
+        return PHASTFT_OK;
+    }
+};
+
 // The Bluestein state of one length L: the chirp w[j] = exp(-pi i (j^2 mod 2L) / L), the transform of the convolution kernel,
 // the M-point plan of both convolution transforms and the workspace, M = 2^ceil(log2(2L - 1)) but at least 4 (Cx16<float>
 // moves two complex values per thread: M = 1 would launch no thread and write past a one-value workspace).  The complex plan
@@ -2287,29 +2348,277 @@ struct Bluestein {
     Plan<T>* inner = nullptr;          // the M-point plan
     cx<T>* chirp = nullptr;            // w[0 .. L), zero-padded to a multiple of Cx16<T>::V
     cx<T>* bhat = nullptr;             // FFT_M(b) / M, computed in f64
-    mutable std::mutex mu;             // the workspace and the owner's host staging
-    mutable cx<T>* ws = nullptr;       // ws_members x M interleaved complex
-    mutable size_t ws_members = 0;
-    mutable cudaEvent_t ws_free = nullptr;   // orders workspace reuse across streams (like Plan::ws_free)
-    mutable cudaStream_t ws_last_stream = nullptr;
-    mutable bool ws_used = false;
+    mutable AnyWorkspace<T> w;         // members x M interleaved complex
     ~Bluestein() {
         if (!inner) return;
         DeviceGuard g(device);
-        if (ws_free) cudaEventDestroy(ws_free);
-        for (void* p : {(void*)chirp, (void*)bhat, (void*)ws})
+        w.destroy();
+        for (void* p : {(void*)chirp, (void*)bhat})
             if (p) cudaFree(p);
         delete inner;
     }
 };
+
+// =================================================================================================
+// any length, smooth N = 2^a 3^b 5^c 7^d: the mixed-radix path (SMOOTH-PRE and the ODD kernels, fft_kernels.cuh)
+// =================================================================================================
+// Lengths on the mixed path stay below 2^30 (a workspace of N values, the exponent of W_N formed in 64 bits).
+constexpr size_t MIXED_MAX_N = (size_t(1) << 30) - 1;
+
+// N = P * Q_a * Q_b: P the power-of-two part, the odd part in one pass (Q_b = 1) or two, each of at most ODD_MAX_ROWS rows.
+struct MixedSplit {
+    size_t p = 0;
+    int qa = 0, qb = 1;
+};
+
+// The split of n, or why it has none (`why` names the offending factor).
+bool mixed_split(size_t n, MixedSplit& out, std::string& why) {
+    if (n < 3 || is_pow2(n)) { why = "n = " + std::to_string(n) + " has no odd factor (powers of two take the c2c plan)"; return false; }
+    if (n > MIXED_MAX_N) { why = "n = " + std::to_string(n) + " is above 2^30 - 1"; return false; }
+    size_t p = 1, q = n;
+    while (q % 2 == 0) { q /= 2; p *= 2; }
+    size_t rest = q;
+    for (size_t f : {3, 5, 7})
+        while (rest % f == 0) rest /= f;
+    if (rest > 1) {
+        size_t f = 11;
+        while (f * f <= rest && rest % f) f += 2;
+        if (rest % f) f = rest;
+        why = "n = " + std::to_string(n) + " has the prime factor " + std::to_string(f) + " (the mixed-radix path takes 2, 3, 5 and 7)";
+        return false;
+    }
+    out.p = p;
+    if (q <= (size_t)ODD_MAX_ROWS) { out.qa = (int)q; out.qb = 1; return true; }
+    size_t best = 0;                                   // the largest divisor a <= sqrt(q): the most balanced split
+    for (size_t a = 3; a * a <= q; a += 2)
+        if (q % a == 0 && q / a <= (size_t)ODD_MAX_ROWS) best = a;
+    if (!best) {
+        why = "n = " + std::to_string(n) + ": its odd part " + std::to_string(q) + " is not a product of two factors of at most " +
+              std::to_string(ODD_MAX_ROWS);
+        return false;
+    }
+    out.qa = (int)best; out.qb = (int)(q / best);
+    return true;
+}
+
+// One ODD pass of R rows: the register kernel for one or two radices up to 35 rows (49 rows of f64 would spill), else the
+// shared-memory tile.
+template <typename T>
+struct OddPass {
+    int r = 0, nstages = 0, rad[ODD_MAX_STAGES] = {};
+    int cw = 0;                        // tile kernel: columns per CTA; 0: the register kernel
+    const cx<T>* wr = nullptr;         // W_R^j (in the plan's table blob)
+    const unsigned short* perm = nullptr;
+};
+
+template <typename T>
+struct Mixed {
+    size_t n = 0;
+    MixedSplit split;
+    int device = 0;
+    Plan<T>* inner = nullptr;          // the P-point plan (it also owns the host calls' stream); nullptr: not built
+    char* tables = nullptr;            // W_N two-level, then per pass W_R and the digit reversal
+    const cx<T>* wn_hi = nullptr;
+    const cx<T>* wn_lo = nullptr;
+    int lo_bits = 0;
+    int npasses = 0;
+    OddPass<T> pass[2];
+    mutable AnyWorkspace<T> w;         // batch x N interleaved complex
+    ~Mixed() {
+        if (!inner) return;
+        DeviceGuard g(device);
+        w.destroy();
+        if (tables) cudaFree(tables);
+        delete inner;
+    }
+};
+
+// radices of an R-row pass, largest first
+inline int odd_stages(int r, int* rad) {
+    int s = 0;
+    for (int f : {7, 5, 3})
+        while (r % f == 0) { r /= f; rad[s++] = f; }
+    return s;
+}
+
+template <typename T>
+int32_t build_mixed(Mixed<T>& mx, size_t n, const MixedSplit& split, int device) {
+    mx.n = n; mx.split = split; mx.device = device;
+    if (int32_t st = build_plan<T>(split.p, device, &mx.inner)) return st;
+    DeviceGuard g(device);
+    int ln = 0;
+    while ((size_t(1) << ln) < n) ++ln;
+    mx.lo_bits = (ln + 1) / 2;
+    const size_t n_lo = size_t(1) << mx.lo_bits, n_hi = ((n - 1) >> mx.lo_bits) + 1;
+    mx.npasses = split.qb > 1 ? 2 : 1;
+    // one blob: every table starts on a 16-byte boundary
+    auto pad = [](size_t b) { return (b + 15) / 16 * 16; };
+    std::vector<char> host;
+    auto append = [&](const void* src, size_t bytes) {
+        const size_t off = host.size();
+        host.resize(off + pad(bytes));
+        memcpy(host.data() + off, src, bytes);
+        return off;
+    };
+    auto roots = [&](size_t count, size_t mul, size_t of) {
+        std::vector<cx<T>> v(count);
+        for (size_t j = 0; j < count; ++j) {
+            double re, im;
+            root_of_unity_any(j * mul, of, re, im);
+            v[j].x = (T)re; v[j].y = (T)im;
+        }
+        return append(v.data(), count * sizeof(cx<T>));
+    };
+    const size_t off_lo = roots(n_lo, 1, n), off_hi = roots(n_hi, n_lo, n);
+    size_t off_wr[2] = {0, 0}, off_perm[2] = {0, 0};
+    for (int i = 0; i < mx.npasses; ++i) {
+        OddPass<T>& ps = mx.pass[i];
+        ps.r = i == 0 ? split.qa : split.qb;
+        ps.nstages = odd_stages(ps.r, ps.rad);
+        off_wr[i] = roots((size_t)ps.r, 1, (size_t)ps.r);
+        if (ps.nstages > 2 || ps.r == 49) {
+            // as many columns as keep the tile under 48 KiB, at least a 128-byte row run
+            const int cmin = 128 / (int)sizeof(cx<T>);
+            ps.cw = ODD_NT;
+            while (ps.cw > cmin && (size_t)ps.r * ps.cw * sizeof(cx<T>) > (size_t(48) << 10)) ps.cw /= 2;
+            // stage 1's butterfly of rows b + q R / rad[0] goes to rows perm[b] rad[0] + q: b's digits, last radix first, reversed
+            std::vector<unsigned short> perm(ps.r / ps.rad[0]);
+            for (size_t b = 0; b < perm.size(); ++b) {
+                size_t m = b, pos = 0, weight = perm.size();
+                for (int s = ps.nstages - 1; s >= 1; --s) {
+                    weight /= ps.rad[s];
+                    pos += m % ps.rad[s] * weight;
+                    m /= ps.rad[s];
+                }
+                perm[b] = (unsigned short)pos;
+            }
+            off_perm[i] = append(perm.data(), perm.size() * sizeof(unsigned short));
+        }
+    }
+    CUDA_TRY(cudaMalloc(&mx.tables, host.size()));
+    CUDA_TRY(cudaMemcpy(mx.tables, host.data(), host.size(), cudaMemcpyHostToDevice));
+    mx.wn_lo = reinterpret_cast<const cx<T>*>(mx.tables + off_lo);
+    mx.wn_hi = reinterpret_cast<const cx<T>*>(mx.tables + off_hi);
+    for (int i = 0; i < mx.npasses; ++i) {
+        mx.pass[i].wr = reinterpret_cast<const cx<T>*>(mx.tables + off_wr[i]);
+        if (mx.pass[i].cw) mx.pass[i].perm = reinterpret_cast<const unsigned short*>(mx.tables + off_perm[i]);
+    }
+    CUDA_TRY(cudaFuncSetAttribute(odd_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  ODD_MAX_ROWS * 128));
+    return mx.w.init(n);                               // room for one member; batched calls grow it
+}
+
+template <typename T, int RA, int RB>
+void launch_odd_reg(const OddParams<T>& q, unsigned grid, cudaStream_t stream) {
+    odd_reg_kernel<T, RA, RB><<<grid, ODD_NT, 0, stream>>>(q);
+}
+
+// One ODD pass over `batch` members.  Launch record: R = rows, C = the columns a CTA covers.
+template <typename T>
+int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cudaStream_t stream) {
+    const OddPass<T>& ps = mx.pass[i];
+    const size_t P = mx.split.p;
+    const bool last = i == mx.npasses - 1;
+    q.role = mx.npasses == 1 ? ODD_SINGLE : i == 0 ? ODD_A : ODD_B;
+    q.r = ps.r; q.qb = mx.split.qb; q.wr = ps.wr; q.perm = ps.perm; q.cw = ps.cw;
+    q.nstages = ps.nstages;
+    for (int s = 0; s < ps.nstages; ++s) q.rad[s] = ps.rad[s];
+    q.cols = (long long)(mx.n / ps.r);
+    q.total = (long long)batch * q.cols;
+    q.in_rs = (long long)(q.role == ODD_A ? mx.split.qb * P : P);
+    q.out_rs = (long long)(q.role == ODD_A ? mx.split.qb * P : q.role == ODD_B ? mx.split.qa * P : P);
+    if (!last) q.scale = T(1);
+    const int cover = ps.cw ? ps.cw : ODD_NT;
+    const size_t blocks = ((size_t)q.total + cover - 1) / cover;
+    if (blocks > 0x7fffffffu) return fail(PHASTFT_ERR_INVALID_ARG, "batch * N is too large for one launch of the odd pass");
+    if (ps.cw) {
+        odd_tile_kernel<T><<<(unsigned)blocks, ODD_NT, (size_t)ps.r * ps.cw * sizeof(cx<T>), stream>>>(q);
+    } else {
+        switch (ps.r) {
+            case 3: launch_odd_reg<T, 3, 1>(q, (unsigned)blocks, stream); break;
+            case 5: launch_odd_reg<T, 5, 1>(q, (unsigned)blocks, stream); break;
+            case 7: launch_odd_reg<T, 7, 1>(q, (unsigned)blocks, stream); break;
+            case 9: launch_odd_reg<T, 3, 3>(q, (unsigned)blocks, stream); break;
+            case 15: launch_odd_reg<T, 5, 3>(q, (unsigned)blocks, stream); break;
+            case 21: launch_odd_reg<T, 7, 3>(q, (unsigned)blocks, stream); break;
+            case 25: launch_odd_reg<T, 5, 5>(q, (unsigned)blocks, stream); break;
+            case 35: launch_odd_reg<T, 7, 5>(q, (unsigned)blocks, stream); break;
+            default: return fail(PHASTFT_ERR_INVALID_ARG, "no register kernel of " + std::to_string(ps.r) + " rows");
+        }
+    }
+    CUDA_TRY(cudaGetLastError());
+    note_launch({"ODD", ps.r, 0, cover, ODD_NT, 0, ps.cw ? "tile" : "reg", false});
+    return PHASTFT_OK;
+}
+
+// One mixed-radix call of `batch` members: SMOOTH-PRE, the P-point plan on Q * batch workspace members, the ODD pass(es).
+// in / out are the caller's planar arrays, swapped for the reverse direction; scale is 1 or 1/N.
+template <typename T>
+int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, T* out_re, T* out_im, size_t bstride, T scale, size_t batch,
+                  cudaStream_t stream) {
+    DeviceGuard g(mx.device);
+    const size_t P = mx.split.p, Q = (size_t)mx.split.qa * mx.split.qb;
+    std::lock_guard<std::mutex> lock(mx.w.mu);
+    bool capturing = false;
+    if (int32_t st = mx.w.acquire(batch * mx.n, batch, stream, "phastft_plan_any_*_reserve", capturing)) return st;
+    SmoothParams<T> sp;
+    sp.in_re = in_re; sp.in_im = in_im; sp.ws = mx.w.ws;
+    sp.n = (long long)mx.n; sp.p = (long long)P; sp.q = (long long)Q; sp.bstride = (long long)bstride;
+    // runs as long as Q and P allow within SMOOTH_TILE values: up to 32 values of n_o, then n_2, then the rest of n_o when P is short
+    size_t tq = std::min<size_t>(Q, 32), tq2 = 1;
+    while (tq2 < tq) tq2 *= 2;
+    const size_t tp = std::min<size_t>(P, SMOOTH_TILE / tq2);
+    if (tp < 32) tq = std::min<size_t>(Q, SMOOTH_TILE / tp);
+    sp.tq = (int)tq; sp.tp = (int)tp;
+    sp.tiles_q = (unsigned)((Q + tq - 1) / tq);
+    sp.tiles_per_member = sp.tiles_q * (unsigned)(P / tp);
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / sp.tiles_per_member);
+    for (size_t done = 0; done < batch; done += max_members) {
+        const size_t nb = std::min(batch - done, max_members);
+        SmoothParams<T> s2 = sp;
+        s2.in_re += done * bstride; s2.in_im += done * bstride; s2.ws += done * mx.n;
+        smooth_pre_kernel<T><<<(unsigned)(nb * sp.tiles_per_member), 256, 0, stream>>>(s2);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({"SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0, "plain", false});
+    }
+    if (P > 1) {
+        Io<T> io;
+        io.in_re = reinterpret_cast<const T*>(mx.w.ws); io.in_im = nullptr;
+        io.out_re = reinterpret_cast<T*>(mx.w.ws); io.out_im = nullptr;
+        io.in_bstride = io.out_bstride = (long long)P;
+        io.in_il = io.out_il = 1;
+        if (int32_t st = run_c2c(*mx.inner, io, Q * batch, T(1), stream)) return st;
+    }
+    OddParams<T> q;
+    memset(&q, 0, sizeof(q));
+    q.ws = mx.w.ws; q.ws_out = mx.w.ws; q.out_re = out_re; q.out_im = out_im;
+    q.wn_hi = mx.wn_hi; q.wn_lo = mx.wn_lo; q.lo_bits = mx.lo_bits;
+    q.n = (long long)mx.n; q.p = (long long)P; q.bstride = (long long)bstride; q.scale = scale;
+    for (int i = 0; i < mx.npasses; ++i)
+        if (int32_t st = launch_odd(mx, i, q, batch, stream)) return st;
+    return mx.w.release(stream, capturing);
+}
+
+// Every allocation a call of `batch` would make: the inner plan's workspace for Q * batch members and batch * N values here.
+template <typename T>
+int32_t mixed_reserve(const Mixed<T>& mx, size_t batch) {
+    if (mx.split.p > 1)
+        if (int32_t st = plan_reserve(mx.inner, (size_t)mx.split.qa * mx.split.qb * batch)) return st;
+    DeviceGuard g(mx.device);
+    std::lock_guard<std::mutex> lock(mx.w.mu);
+    return mx.w.grow(batch * mx.n, batch);
+}
 
 template <typename T>
 struct PlanAny {
     size_t n = 0;
     int device = 0;
     Plan<T>* pow2 = nullptr;           // N a power of two: the N-point plan, run as it is
-    Bluestein<T> bs;                   // otherwise: Bluestein of L = N
-    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then bs.mu)
+    Bluestein<T> bs;                   // otherwise: Bluestein of L = N ...
+    Mixed<T> mx;                       // ... or the mixed-radix path (mx.inner set)
+    AnyWorkspace<T>& workspace() const { return mx.inner ? mx.w : bs.w; }
+    cudaStream_t host_stream() const { return (mx.inner ? mx.inner : bs.inner)->stream; }
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then the workspace's mu)
     mutable T* stage_re = nullptr;     // host-API staging: N each
     mutable T* stage_im = nullptr;
     std::string description;
@@ -2409,19 +2718,22 @@ int32_t build_bluestein(Bluestein<T>& bs, size_t l, int device) {
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaDeviceSynchronize());
     }
-    CUDA_TRY(cudaMalloc(&bs.ws, M * sizeof(cx<T>)));                 // room for one member; batched calls grow it
-    bs.ws_members = 1;
-    CUDA_TRY(cudaEventCreateWithFlags(&bs.ws_free, cudaEventDisableTiming));
-    return PHASTFT_OK;
+    return bs.w.init(M);                                             // room for one member; batched calls grow it
 }
 
 template <typename T>
-int32_t build_plan_any(size_t n, int device, PlanAny<T>** out) {
+int32_t build_plan_any(size_t n, int device, int algo, PlanAny<T>** out) {
     if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
     *out = nullptr;
     if (n == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n must be >= 1");
+    if (algo != PHASTFT_ANY_BLUESTEIN && algo != PHASTFT_ANY_MIXED && algo != PHASTFT_ANY_AUTO)
+        return fail(PHASTFT_ERR_INVALID_ARG, "algo must be PHASTFT_ANY_BLUESTEIN, PHASTFT_ANY_MIXED or PHASTFT_ANY_AUTO");
     const bool pow2 = is_pow2(n);
-    if (!pow2 && n > ANY_MAX_N)
+    MixedSplit split;
+    std::string why;
+    const bool mixed = !pow2 && algo != PHASTFT_ANY_BLUESTEIN && mixed_split(n, split, why);
+    if (!pow2 && algo == PHASTFT_ANY_MIXED && !mixed) return fail(PHASTFT_ERR_INVALID_ARG, "no mixed-radix plan: " + why);
+    if (!pow2 && !mixed && n > ANY_MAX_N)
         return fail(PHASTFT_ERR_INVALID_ARG, "n = " + std::to_string(n) + " is not a power of two and above 2^29 - 1 (its convolution "
                                              "length 2^ceil(log2(2N - 1)) would exceed 2^30)");
     std::unique_ptr<PlanAny<T>> pl(new PlanAny<T>());
@@ -2430,6 +2742,14 @@ int32_t build_plan_any(size_t n, int device, PlanAny<T>** out) {
     if (pow2) {
         if (int32_t st = build_plan<T>(n, device, &pl->pow2)) return st;
         pl->description = "n=2^" + std::to_string(ilog2(n)) + prec + " any: power of two | inner: " + pl->pow2->description;
+        *out = pl.release();
+        return PHASTFT_OK;
+    }
+    if (mixed) {
+        if (int32_t st = build_mixed(pl->mx, n, split, device)) return st;
+        pl->description = "n=" + std::to_string(n) + prec + " any: mixed 2^" + std::to_string(ilog2(split.p)) + " x " +
+                          std::to_string(split.qa) + (split.qb > 1 ? " x " + std::to_string(split.qb) : "") + " | inner: " +
+                          pl->mx.inner->description;
         *out = pl.release();
         return PHASTFT_OK;
     }
@@ -2477,47 +2797,22 @@ int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_
     return PHASTFT_OK;
 }
 
-// Grows the workspace to `members` x M.  Caller holds bs.mu.  The new array is allocated before the old one is released, so a
-// failed allocation leaves the plan as it was.
-template <typename T>
-int32_t grow_bluestein_workspace(const Bluestein<T>& bs, size_t members) {
-    if (bs.ws_members >= members) return PHASTFT_OK;
-    cx<T>* w = nullptr;
-    if (cudaMalloc(&w, (members << bs.log2m) * sizeof(cx<T>)) != cudaSuccess) {
-        (void)cudaGetLastError();
-        return fail(PHASTFT_ERR_CUDA, "cudaMalloc of the plan's workspace for " + std::to_string(members) + " members failed");
-    }
-    CUDA_TRY(cudaDeviceSynchronize());   // every earlier user of the old workspace, on any stream, is done
-    cudaFree(bs.ws);
-    bs.ws = w; bs.ws_members = members;
-    return PHASTFT_OK;
-}
-
 // One Bluestein call of `batch` members: CHIRP-PRE, the M-point transform, CHIRP-MUL, the M-point transform, CHIRP-POST, with
 // the kernels' MODE at both ends.  `cp` carries the caller's arrays, strides, scale and W_N table; this fills in the rest.  The
-// workspace protocol of run_c2c: grown (synchronising) outside a capture only (`reserve_fn` names the call that grows it
-// ahead); a caller on another stream first waits for the previous user.
+// workspace follows AnyWorkspace's protocol (`reserve_fn` names the call that grows it ahead of a capture).
 template <int MODE, typename T>
 int32_t bluestein_run(const Bluestein<T>& bs, ChirpParams<T> cp, size_t batch, cudaStream_t stream, const char* reserve_fn) {
     DeviceGuard g(bs.device);
     const size_t M = size_t(1) << bs.log2m;
-    std::lock_guard<std::mutex> lock(bs.mu);
-    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-    CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
-    const bool capturing = cap != cudaStreamCaptureStatusNone;
-    if (bs.ws_members < batch) {
-        if (capturing)
-            return fail(PHASTFT_ERR_INVALID_ARG, std::string("the plan's workspace is too small for this batch and the stream is being "
-                                                             "captured: call ") + reserve_fn + "(batch) before capturing");
-        if (int32_t st = grow_bluestein_workspace(bs, batch)) return st;
-    }
-    if (!capturing && bs.ws_used && bs.ws_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, bs.ws_free, 0));
-    cp.ws = bs.ws; cp.chirp = bs.chirp; cp.bhat = bs.bhat;
+    std::lock_guard<std::mutex> lock(bs.w.mu);
+    bool capturing = false;
+    if (int32_t st = bs.w.acquire(batch << bs.log2m, batch, stream, reserve_fn, capturing)) return st;
+    cp.ws = bs.w.ws; cp.chirp = bs.chirp; cp.bhat = bs.bhat;
     cp.n = (long long)bs.l; cp.log2m = bs.log2m;
     constexpr size_t V = Cx16<T>::V;
     Io<T> io;
-    io.in_re = reinterpret_cast<const T*>(bs.ws); io.in_im = nullptr;
-    io.out_re = reinterpret_cast<T*>(bs.ws); io.out_im = nullptr;
+    io.in_re = reinterpret_cast<const T*>(bs.w.ws); io.in_im = nullptr;
+    io.out_re = reinterpret_cast<T*>(bs.w.ws); io.out_im = nullptr;
     io.in_bstride = io.out_bstride = (long long)M;
     io.in_il = io.out_il = 1;
     const size_t post = (size_t)chirp_post_count<MODE>((long long)bs.l);
@@ -2526,12 +2821,7 @@ int32_t bluestein_run(const Bluestein<T>& bs, ChirpParams<T> cp, size_t batch, c
     if (int32_t st = launch_chirp<MODE>(CHIRP_MUL, cp, M / V, batch, stream)) return st;
     if (int32_t st = run_c2c(*bs.inner, io, batch, T(1), stream)) return st;
     if (int32_t st = launch_chirp<MODE>(CHIRP_POST, cp, (post + V - 1) / V, batch, stream)) return st;
-    if (!capturing) {
-        CUDA_TRY(cudaEventRecord(bs.ws_free, stream));
-        bs.ws_last_stream = stream;
-        bs.ws_used = true;
-    }
-    return PHASTFT_OK;
+    return bs.w.release(stream, capturing);
 }
 
 // Every allocation a call of `batch` would make: the inner plan's workspace and the Bluestein one.
@@ -2539,8 +2829,8 @@ template <typename T>
 int32_t bluestein_reserve(const Bluestein<T>& bs, size_t batch) {
     if (int32_t st = plan_reserve(bs.inner, batch)) return st;
     DeviceGuard g(bs.device);
-    std::lock_guard<std::mutex> lock(bs.mu);
-    return grow_bluestein_workspace(bs, batch);
+    std::lock_guard<std::mutex> lock(bs.w.mu);
+    return bs.w.grow(batch << bs.log2m, batch);
 }
 
 // planar, in place, device pointers: the semantics of fft_dev for any N
@@ -2553,6 +2843,9 @@ int32_t any_dev(const PlanAny<T>* pl, T* d_re, T* d_im, int direction, size_t ba
     if (batch == 0) return PHASTFT_OK;
     // the reverse direction by the swap trick (fft_dev): re and im exchanged on the way in and out, 1/N folded into CHIRP-POST
     const bool fwd = direction == PHASTFT_FORWARD;
+    if (pl->mx.inner)
+        return mixed_run(pl->mx, fwd ? d_re : d_im, fwd ? d_im : d_re, fwd ? d_re : d_im, fwd ? d_im : d_re, bstride,
+                         fwd ? T(1) : T(1) / (T)pl->n, batch, stream);
     ChirpParams<T> cp;
     memset(&cp, 0, sizeof(cp));
     cp.in_re = cp.out_re = fwd ? d_re : d_im;
@@ -2566,6 +2859,7 @@ template <typename T>
 int32_t any_reserve(const PlanAny<T>* pl, size_t batch) {
     if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
     if (pl->pow2) return plan_reserve(pl->pow2, batch);
+    if (pl->mx.inner) return mixed_reserve(pl->mx, batch);
     return bluestein_reserve(pl->bs, batch);
 }
 
@@ -2581,11 +2875,11 @@ int32_t any_host(const PlanAny<T>* pl, T* re, size_t len_re, T* im, size_t len_i
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> host_lock(pl->host_mu);
     {
-        std::lock_guard<std::mutex> lock(pl->bs.mu);    // released before any_dev, which takes it
+        std::lock_guard<std::mutex> lock(pl->workspace().mu);   // released before any_dev, which takes it
         if (!pl->stage_re) CUDA_TRY(cudaMalloc(&pl->stage_re, pl->n * sizeof(T)));
         if (!pl->stage_im) CUDA_TRY(cudaMalloc(&pl->stage_im, pl->n * sizeof(T)));
     }
-    cudaStream_t s = pl->bs.inner->stream;
+    cudaStream_t s = pl->host_stream();
     const size_t bytes = pl->n * sizeof(T);
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, re, bytes, cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_im, im, bytes, cudaMemcpyHostToDevice, s));
@@ -2611,7 +2905,7 @@ struct PlanR2cAny {
     PlanR2c<T>* pow2 = nullptr;        // N a power of two >= 4: the r2c plan, run as it is
     Bluestein<T> bs;
     cx<T>* wn = nullptr;               // halved: W_N^k for k = 0 .. floor(L/2), rounded to T
-    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then bs.mu)
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then the workspace's mu)
     mutable T* stage_real = nullptr;   // host-API staging: N reals, floor(N/2) + 1 bins
     mutable T* stage_re = nullptr;
     mutable T* stage_im = nullptr;
@@ -2742,7 +3036,7 @@ int32_t r2c_any_reserve(const PlanR2cAny<T>* pl, size_t batch) {
 // Caller holds host_mu.
 template <typename T>
 int32_t ensure_r2c_any_staging(const PlanR2cAny<T>* pl) {
-    std::lock_guard<std::mutex> lock(pl->bs.mu);         // released before the device call, which takes it
+    std::lock_guard<std::mutex> lock(pl->bs.w.mu);       // released before the device call, which takes it
     if (!pl->stage_real) CUDA_TRY(cudaMalloc(&pl->stage_real, pl->n * sizeof(T)));
     if (!pl->stage_re) CUDA_TRY(cudaMalloc(&pl->stage_re, (pl->n / 2 + 1) * sizeof(T)));
     if (!pl->stage_im) CUDA_TRY(cudaMalloc(&pl->stage_im, (pl->n / 2 + 1) * sizeof(T)));
@@ -2856,6 +3150,15 @@ int32_t phastft_plan_factorization(size_t n, int precision_bits, int* log2_facto
     std::vector<int> f = ln == 0 ? std::vector<int>{} : (precision_bits == 64 ? choose_factors<double>(ln) : choose_factors<float>(ln));
     *num_passes = (int)f.size();
     for (size_t i = 0; i < f.size(); ++i) log2_factors[i] = f[i];
+    return PHASTFT_OK;
+}
+
+int32_t phastft_any_mixed_factorization(size_t n, size_t* p, int* q_a, int* q_b) {
+    if (!p || !q_a || !q_b) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
+    MixedSplit s;
+    std::string why;
+    if (!mixed_split(n, s, why)) return fail(PHASTFT_ERR_INVALID_ARG, "no mixed-radix plan: " + why);
+    *p = s.p; *q_a = s.qa; *q_b = s.qb;
     return PHASTFT_OK;
 }
 
@@ -3021,7 +3324,14 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     }                                                                                                                   \
     int32_t phastft_plan_any_##SFX##_create(size_t n, int device, phastft_plan_any_##SFX** out) {                       \
         PlanAny<T>* pl = nullptr;                                                                                       \
-        int32_t st = build_plan_any<T>(n, device, &pl);                                                                 \
+        int32_t st = build_plan_any<T>(n, device, PHASTFT_ANY_BLUESTEIN, &pl);                                          \
+        if (out) *out = reinterpret_cast<phastft_plan_any_##SFX*>(pl);                                                  \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    int32_t phastft_plan_any_##SFX##_create_with(size_t n, int device, int algo, phastft_plan_any_##SFX** out) {        \
+        PlanAny<T>* pl = nullptr;                                                                                       \
+        int32_t st = build_plan_any<T>(n, device, algo, &pl);                                                           \
         if (out) *out = reinterpret_cast<phastft_plan_any_##SFX*>(pl);                                                  \
         else if (pl) delete pl;                                                                                         \
         return st;                                                                                                      \

@@ -98,8 +98,18 @@ impl_planner_r2c!(PlannerR2c64, ffi::phastft_plan_r2c_f64, phastft_plan_r2c_f64_
 impl_planner_r2c!(PlannerR2c32, ffi::phastft_plan_r2c_f32, phastft_plan_r2c_f32_create, phastft_plan_r2c_f32_destroy,
                   phastft_plan_r2c_f32_reserve);
 
+/// How a length that is not a power of two is transformed (`PHASTFT_ANY_*`).  `Auto` takes `Mixed` for every eligible length
+/// (2^a 3^b 5^c 7^d below 2^30 whose odd part fits one or two odd passes) and `Bluestein` otherwise, from the factorisation alone.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum AnyAlgo {
+    Bluestein = 0,
+    Mixed = 1,
+    Auto = 2,
+}
+
 macro_rules! impl_planner_any {
-    ($name:ident, $raw:ty, $create:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
+    ($name:ident, $raw:ty, $create:ident, $create_with:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
         /// Additive (the reference accepts powers of two only): a complex FFT of any length.  A power of two runs the c2c plan
         /// as it is; any other length up to 2^29 - 1 runs Bluestein's algorithm over a power-of-two plan.
         pub struct $name {
@@ -114,11 +124,17 @@ macro_rules! impl_planner_any {
                 check(unsafe { ffi::$create(num_points, device(), &mut raw) });
                 Self { raw }
             }
+            /// `new` with the algorithm chosen.  Panics as `new` does, and for `AnyAlgo::Mixed` on a length that is not eligible.
+            pub fn with_algo(num_points: usize, algo: AnyAlgo) -> Self {
+                let mut raw = std::ptr::null_mut();
+                check(unsafe { ffi::$create_with(num_points, device(), algo as std::os::raw::c_int, &mut raw) });
+                Self { raw }
+            }
             /// Number of points the planner was built for.
             pub fn num_points(&self) -> usize {
                 unsafe { ffi::$size(self.raw) }
             }
-            /// `"n=1000 f64 any: Bluestein M=2^11 | inner: ..."` or `"n=2^20 f64 any: power of two | inner: ..."`.
+            /// `"n=1000 f64 any: Bluestein M=2^11 | inner: ..."`, `"n=1000 f64 any: mixed 2^3 x 125 | inner: ..."` or `"n=2^20 f64 any: power of two | inner: ..."`.
             pub fn describe(&self) -> String {
                 unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
             }
@@ -134,9 +150,9 @@ macro_rules! impl_planner_any {
         }
     };
 }
-impl_planner_any!(PlannerAny64, ffi::phastft_plan_any_f64, phastft_plan_any_f64_create, phastft_plan_any_f64_destroy,
+impl_planner_any!(PlannerAny64, ffi::phastft_plan_any_f64, phastft_plan_any_f64_create, phastft_plan_any_f64_create_with, phastft_plan_any_f64_destroy,
                   phastft_plan_any_f64_size, phastft_plan_any_f64_describe, phastft_plan_any_f64_reserve);
-impl_planner_any!(PlannerAny32, ffi::phastft_plan_any_f32, phastft_plan_any_f32_create, phastft_plan_any_f32_destroy,
+impl_planner_any!(PlannerAny32, ffi::phastft_plan_any_f32, phastft_plan_any_f32_create, phastft_plan_any_f32_create_with, phastft_plan_any_f32_destroy,
                   phastft_plan_any_f32_size, phastft_plan_any_f32_describe, phastft_plan_any_f32_reserve);
 
 macro_rules! impl_planner_r2c_any {
