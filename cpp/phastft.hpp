@@ -78,7 +78,7 @@ template <> struct Api<double> {
     static int32_t any_dev(const Any* p, double* re, double* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f64_dev(p, re, im, d, b, st, s); }
     static int32_t any_host(const Any* p, double* re, std::size_t lr, double* im, std::size_t li, int d) { return phastft_fft_any_f64_host(p, re, lr, im, li, d); }
     using R2cAny = phastft_plan_r2c_any_f64;
-    static int32_t r2c_any_create(std::size_t n, int dev, R2cAny** o) { return phastft_plan_r2c_any_f64_create(n, dev, o); }
+    static int32_t r2c_any_create(std::size_t n, int dev, int algo, R2cAny** o) { return phastft_plan_r2c_any_f64_create_with(n, dev, algo, o); }
     static void r2c_any_destroy(R2cAny* p) { phastft_plan_r2c_any_f64_destroy(p); }
     static std::size_t r2c_any_size(const R2cAny* p) { return phastft_plan_r2c_any_f64_size(p); }
     static const char* r2c_any_describe(const R2cAny* p) { return phastft_plan_r2c_any_f64_describe(p); }
@@ -117,7 +117,7 @@ template <> struct Api<float> {
     static int32_t any_dev(const Any* p, float* re, float* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f32_dev(p, re, im, d, b, st, s); }
     static int32_t any_host(const Any* p, float* re, std::size_t lr, float* im, std::size_t li, int d) { return phastft_fft_any_f32_host(p, re, lr, im, li, d); }
     using R2cAny = phastft_plan_r2c_any_f32;
-    static int32_t r2c_any_create(std::size_t n, int dev, R2cAny** o) { return phastft_plan_r2c_any_f32_create(n, dev, o); }
+    static int32_t r2c_any_create(std::size_t n, int dev, int algo, R2cAny** o) { return phastft_plan_r2c_any_f32_create_with(n, dev, algo, o); }
     static void r2c_any_destroy(R2cAny* p) { phastft_plan_r2c_any_f32_destroy(p); }
     static std::size_t r2c_any_size(const R2cAny* p) { return phastft_plan_r2c_any_f32_size(p); }
     static const char* r2c_any_describe(const R2cAny* p) { return phastft_plan_r2c_any_f32_describe(p); }
@@ -212,17 +212,21 @@ class PlannerAny {
 };
 
 /// additive: real-input FFTs of any length (a power of two >= 4 runs the r2c plan; an even length up to 2^30 - 2 Bluestein of
-/// N/2, an odd one up to 2^29 - 1 Bluestein of N)
+/// N/2, an odd one up to 2^29 - 1 Bluestein of N, or with AnyAlgo::Mixed / AnyAlgo::Auto the mixed-radix path of N/2 or N when
+/// that length is eligible)
 template <typename T>
 class PlannerR2cAny {
   public:
-    explicit PlannerR2cAny(std::size_t n, int device = 0) { check(Api<T>::r2c_any_create(n, device, &raw_)); }
+    explicit PlannerR2cAny(std::size_t n, int device = 0, AnyAlgo algo = AnyAlgo::Bluestein) {
+        check(Api<T>::r2c_any_create(n, device, static_cast<int>(algo), &raw_));
+    }
     ~PlannerR2cAny() { if (raw_) Api<T>::r2c_any_destroy(raw_); }
     PlannerR2cAny(PlannerR2cAny&& o) noexcept : raw_(o.raw_) { o.raw_ = nullptr; }
     PlannerR2cAny(const PlannerR2cAny&) = delete;
     PlannerR2cAny& operator=(const PlannerR2cAny&) = delete;
     std::size_t n() const { return Api<T>::r2c_any_size(raw_); }
-    /// "power of two", or "halved" / "direct" with the Bluestein length and M, then the inner plan's description
+    /// "power of two", or "halved" / "direct" with "Bluestein L=<L> M=2^m" or "mixed 2^a x Q_a[ x Q_b]", then the inner plan's
+    /// description
     std::string describe() const { return Api<T>::r2c_any_describe(raw_); }
     /// make every allocation a call of `batch` members would make now
     void reserve(std::size_t batch) const { check(Api<T>::r2c_any_reserve(raw_, batch)); }

@@ -49,7 +49,9 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * kernels), CHIRP-PRE / CHIRP-MUL / CHIRP-POST (the any-length transform's elementwise kernels: R=<M>, C=<members>), CHIRP-PRE-R2C /
  * CHIRP-POST-R2C / CHIRP-PRE-C2R / CHIRP-POST-C2R (the same around the real any-length transforms), SMOOTH-PRE (the mixed-radix
  * path's de-interleave: R=<P>, C=<workspace members>) and ODD (its radix-3/5/7 passes: R=<rows>, C=<columns per CTA>, mode reg
- * for the register kernel or tile for the shared-memory one); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * for the register kernel or tile for the shared-memory one), SMOOTH-PRE-R2C / SMOOTH-PRE-C2R and ODD-R2C / ODD-C2R (the same with
+ * the real any-length transforms' loads and last-pass stores) and SMOOTH-POST-R2C (their halved r2c's untangle: R=<L>,
+ * C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
@@ -335,6 +337,19 @@ PHASTFT_API int32_t phastft_fft_any_f32_host(const phastft_plan_any_f32* plan, f
  * The Bluestein paths run CHIRP-PRE-R2C / CHIRP-POST-R2C (CHIRP-PRE-C2R / CHIRP-POST-C2R) around the two M-point transforms
  * and CHIRP-MUL of the complex any-length plan.  Any other n returns PHASTFT_ERR_INVALID_ARG at create, before the device is
  * touched.
+ * phastft_plan_r2c_any_*_create_with(n, device, algo, out) selects the algorithm of the halved and direct paths with the
+ * PHASTFT_ANY_* values of the complex plan (powers of two take the r2c plan under every value; _create builds Bluestein):
+ *   PHASTFT_ANY_MIXED   the mixed-radix path of L = n/2 (halved, even n up to 2^31 - 2) or of L = n (direct, odd n = Q_a * Q_b
+ *                       <= 729^2): SMOOTH-PRE-R2C loads the pairs (or the reals) into the workspace, the P-point plan and the ODD
+ *                       passes transform it; the halved r2c stores Z = DFT_L(z) into the bins and SMOOTH-POST-R2C untangles them
+ *                       in place with W_n^k, the direct r2c's last pass (ODD-R2C) stores bins 0 .. floor(n/2) only.  c2r loads
+ *                       the c2r pre-processing with W_n^m (halved) or the Hermitian extension (direct) in SMOOTH-PRE-C2R, and the
+ *                       last pass (ODD-C2R) stores the pairs (y[2k], y[2k+1]) or the real part.  No padding.  An n whose L is
+ *                       not eligible for phastft_any_mixed_factorization returns PHASTFT_ERR_INVALID_ARG (the detail names L or
+ *                       n and the reason) before the device is touched.
+ *   PHASTFT_ANY_AUTO    mixed when L is eligible, Bluestein otherwise (an even n above 2^30 - 2 that is not eligible is refused).
+ * describe(): "n=44100 f64 r2c any: halved, mixed 2^1 x 105 x 105 | inner: ..." or "n=1125 f64 r2c any: direct, mixed 2^0 x 25 x 45 |
+ * inner: ...".
  * c2r of a spectrum that is not the half-spectrum of a real signal (non-real X[0], or for even n non-real X[n/2]): even n uses
  * the c2r pre-processing formula with W_n, as the power-of-two c2r does; odd n uses the Hermitian extension
  * Y[m] = conj X[n - m] (m > n/2) and keeps the real part of the inverse, so Im X[0] is dropped, as numpy.fft.irfft does.
@@ -343,6 +358,8 @@ typedef struct phastft_plan_r2c_any_f64 phastft_plan_r2c_any_f64;
 typedef struct phastft_plan_r2c_any_f32 phastft_plan_r2c_any_f32;
 PHASTFT_API int32_t phastft_plan_r2c_any_f64_create(size_t n, int device, phastft_plan_r2c_any_f64** out);
 PHASTFT_API int32_t phastft_plan_r2c_any_f32_create(size_t n, int device, phastft_plan_r2c_any_f32** out);
+PHASTFT_API int32_t phastft_plan_r2c_any_f64_create_with(size_t n, int device, int algo, phastft_plan_r2c_any_f64** out);
+PHASTFT_API int32_t phastft_plan_r2c_any_f32_create_with(size_t n, int device, int algo, phastft_plan_r2c_any_f32** out);
 PHASTFT_API void phastft_plan_r2c_any_f64_destroy(phastft_plan_r2c_any_f64* plan);
 PHASTFT_API void phastft_plan_r2c_any_f32_destroy(phastft_plan_r2c_any_f32* plan);
 PHASTFT_API size_t phastft_plan_r2c_any_f64_size(const phastft_plan_r2c_any_f64* plan);

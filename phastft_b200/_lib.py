@@ -115,6 +115,7 @@ SIGNATURES = {
     "phastft_fft_any_{s}_dev": ([_vp, _vp, _vp, _ci, _sz, _sz, _vp], _i32),
     "phastft_fft_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _ci], _i32),
     "phastft_plan_r2c_any_{s}_create": ([_sz, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_r2c_any_{s}_create_with": ([_sz, _ci, _ci, C.POINTER(_vp)], _i32),
     "phastft_plan_r2c_any_{s}_destroy": ([_vp], None),
     "phastft_plan_r2c_any_{s}_size": ([_vp], _sz),
     "phastft_plan_r2c_any_{s}_describe": ([_vp], C.c_char_p),

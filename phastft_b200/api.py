@@ -291,22 +291,28 @@ class _PlannerR2cAny:
     _sfx = ""
     _dtype = None
 
-    def __init__(self, n: int, device: int = 0):
+    def __init__(self, n: int, device: int = 0, algo: AnyAlgo = AnyAlgo.Bluestein):
         """Real-input FFTs of any length n (the reference's r2c accepts powers of two >= 4 only): a power of two from 4 to
         2^31 runs the r2c plan as it is, an even n up to 2^30 - 2 Bluestein of n/2 ("halved"), an odd n up to 2^29 - 1
-        Bluestein of n ("direct").  Other lengths raise PhastFTPanic(13) before the device is touched."""
+        Bluestein of n ("direct").  With AnyAlgo.Mixed / AnyAlgo.Auto the halved and direct paths run the mixed-radix
+        transform of n/2 (even n up to 2^31 - 2) or n instead when that length is eligible.  Other lengths (and
+        AnyAlgo.Mixed on a length that is not eligible) raise PhastFTPanic(13) before the device is touched."""
         self._h = C.c_void_p()
         self.device = int(device)
-        check(fn("phastft_plan_r2c_any_{s}_create", self._sfx)(int(n), self.device, C.byref(self._h)))
+        check(fn("phastft_plan_r2c_any_{s}_create_with", self._sfx)(int(n), self.device, int(algo), C.byref(self._h)))
         self.n = int(n)
 
     @classmethod
     def new(cls, n: int, device: int = 0):
         return cls(n, device)
 
+    @classmethod
+    def with_algo(cls, n: int, algo: AnyAlgo, device: int = 0):
+        return cls(n, device, algo)
+
     def describe(self) -> str:
-        """"power of two | <the r2c plan's describe()>", or "halved" / "direct", the Bluestein length and M, then the inner
-        plan's describe()."""
+        """"power of two | <the r2c plan's describe()>", or "halved" / "direct", then "Bluestein L=<L> M=2^m" or
+        "mixed 2^a x Q_a[ x Q_b]", then the inner plan's describe()."""
         return fn("phastft_plan_r2c_any_{s}_describe", self._sfx)(self._h).decode()
 
     def reserve(self, batch: int) -> None:

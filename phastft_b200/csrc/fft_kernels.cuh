@@ -970,6 +970,38 @@ __device__ __forceinline__ cx<T> chirp_wn(const ChirpParams<T>& p, long long k) 
     return make_cx<T>(-w.x, w.y);
 }
 
+// The real modes' arithmetic at the two ends, shared by the Bluestein (CHIRP-*) and mixed-radix (SMOOTH-* / ODD) kernels.
+// c2r_preprocess_kernel's formula with w = W_N^m, L = N/2 bins in re / im: z = (X[m] + conj X[L-m]) / 2 +
+// i conj(w) (X[m] - conj X[L-m]) / 2, swapped for the inverse
+template <typename T>
+__device__ __forceinline__ cx<T> c2r_halved_in(const T* re, const T* im, long long l, long long m, cx<T> w) {
+    const long long s = l - m;
+    const T c_h = T(0.5) * w.x, s_h = T(0.5) * w.y;
+    const T re_f = re[m], im_f = im[m], re_s = re[s], im_s = -im[s];
+    const T zx_re = T(0.5) * (re_f + re_s), zx_im = T(0.5) * (im_f + im_s);
+    const T dr = re_f - re_s, di = im_f - im_s;
+    const T zy_re = c_h * dr + s_h * di;
+    const T zy_im = c_h * di - s_h * dr;
+    return make_cx<T>(zx_im + zy_re, zx_re - zy_im);
+}
+// odd N: the Hermitian extension Y[m] = X[m] (m <= N/2) or conj X[N - m], swapped
+template <typename T>
+__device__ __forceinline__ cx<T> c2r_direct_in(const T* re, const T* im, long long n, long long m) {
+    return 2 * m <= n ? make_cx<T>(im[m], re[m]) : make_cx<T>(-im[n - m], re[n - m]);
+}
+// r2c_untangle_kernel's formula for the bin pair (k, L - k) of Z = DFT_L(z), w = W_N^k: X[k] and X[L - k]
+template <typename T>
+__device__ __forceinline__ void r2c_untangle(cx<T> zk, cx<T> zm, cx<T> w, cx<T>& xk, cx<T>& xm) {
+    const T wkr = T(0.5) * w.x, wki = T(0.5) * w.y;
+    const T a = zk.x, b = zk.y, cc = zm.x, d = zm.y;
+    const T s_re = T(0.5) * (a + cc), s_im = T(0.5) * (b - d);
+    const T t_re = b + d, t_im = cc - a;
+    const T wzr = wkr * t_re - wki * t_im;
+    const T wzi = wkr * t_im + wki * t_re;
+    xk = make_cx<T>(s_re + wzr, s_im + wzi);
+    xm = make_cx<T>(s_re - wzr, wzi - s_im);
+}
+
 // CHIRP-PRE's value before the chirp product, real modes: member mb's element m < L
 template <typename T, int MODE>
 __device__ __forceinline__ cx<T> chirp_real_in(const ChirpParams<T>& p, unsigned mb, long long m) {
@@ -978,21 +1010,8 @@ __device__ __forceinline__ cx<T> chirp_real_in(const ChirpParams<T>& p, unsigned
         return reinterpret_cast<const cx<T>*>(re)[m];                   // (x[2m], x[2m+1]): base and stride keep pairs aligned
     } else {
         const T* im = p.in_im + (long long)mb * p.bstride;
-        if constexpr (MODE == CHIRP_C2R_HALVED) {
-            // c2r_preprocess_kernel's formula with W_N^m: z = (X[m] + conj X[L-m]) / 2 + i conj(W_N^m) (X[m] - conj X[L-m]) / 2
-            const long long s = p.n - m;
-            const cx<T> w = chirp_wn(p, m);
-            const T c_h = T(0.5) * w.x, s_h = T(0.5) * w.y;
-            const T re_f = re[m], im_f = im[m], re_s = re[s], im_s = -im[s];
-            const T zx_re = T(0.5) * (re_f + re_s), zx_im = T(0.5) * (im_f + im_s);
-            const T dr = re_f - re_s, di = im_f - im_s;
-            const T zy_re = c_h * dr + s_h * di;
-            const T zy_im = c_h * di - s_h * dr;
-            return make_cx<T>(zx_im + zy_re, zx_re - zy_im);           // swapped for the inverse
-        } else {
-            // Y[m] = X[m] (m <= N/2) or conj X[N - m], swapped
-            return 2 * m <= p.n ? make_cx<T>(im[m], re[m]) : make_cx<T>(-im[p.n - m], re[p.n - m]);
-        }
+        if constexpr (MODE == CHIRP_C2R_HALVED) return c2r_halved_in<T>(re, im, p.n, m, chirp_wn(p, m));
+        else return c2r_direct_in<T>(re, im, p.n, m);
     }
 }
 
@@ -1091,15 +1110,10 @@ __global__ void __launch_bounds__(256) chirp_post_kernel(const __grid_constant__
             const cx<T> zk = cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y));
             const cx<T> cm = ws[mm], wm = p.chirp[mm];
             const cx<T> zm = cmul<T>(wm, make_cx<T>(cm.x, -cm.y));
-            const cx<T> wn = p.wn[k];
-            const T wkr = T(0.5) * wn.x, wki = T(0.5) * wn.y;
-            const T a = zk.x, b = zk.y, cc = zm.x, d = zm.y;
-            const T s_re = T(0.5) * (a + cc), s_im = T(0.5) * (b - d);
-            const T t_re = b + d, t_im = cc - a;
-            const T wzr = wkr * t_re - wki * t_im;
-            const T wzi = wkr * t_im + wki * t_re;
-            re[k] = s_re + wzr; im[k] = s_im + wzi;
-            if (m != k) { re[m] = s_re - wzr; im[m] = wzi - s_im; }
+            cx<T> xk, xm;
+            r2c_untangle<T>(zk, zm, p.wn[k], xk, xm);
+            re[k] = xk.x; im[k] = xk.y;
+            if (m != k) { re[m] = xm.x; im[m] = xm.y; }
         }
     } else if constexpr (MODE == CHIRP_R2C_DIRECT) {
         T* re = p.out_re + (long long)mb * p.out_bstride;
@@ -1149,6 +1163,10 @@ __global__ void __launch_bounds__(256) chirp_narrow_kernel(const double2* __rest
 //               in the workspace, rows Q_b P apart), pass B (W_Q^(n_b k_a) on load, n_b -> k_b, planar store of row k_a + Q_a k_b).
 // Every pass is "R rows, N / R columns per member": column c of member m reads rows r at in0 + r * in_rs, multiplies by
 // W_N^(e0 + r * de) and writes row k at c + k * out_rs.
+// The real any-length plan runs the same kernels with a ChirpMode at both ends (N below is the mixed length: L = N_real / 2
+// for the halved modes, N_real for the direct ones): SMOOTH-PRE loads what CHIRP-PRE would (the pairs, the real data, the c2r
+// pre-processing with W_(2L)^m, the Hermitian extension), the last ODD pass stores the pairs, the real part or the bins up to
+// floor(N/2), and the halved r2c untangles the bins in place afterwards (SMOOTH-POST-R2C).  Pass A is always C2C.
 // ---------------------------------------------------------------------------------------------
 enum OddRole { ODD_SINGLE, ODD_A, ODD_B };
 constexpr int ODD_MAX_STAGES = 6;      // 3^6 = 729
@@ -1174,13 +1192,16 @@ struct OddParams {
     T scale;                       // the last pass: 1 forward, 1/N reverse
 };
 
-// One column of a pass: where its rows are, its twiddle exponents and where its output rows go.
-template <typename T>
+// One column of a pass: where its rows are, its twiddle exponents and where its output rows go.  MODE: how the last pass
+// stores (C2C for pass A).
+template <typename T, int MODE = CHIRP_C2C>
 struct OddCol {
     const cx<T>* in;
     cx<T>* out_c;
     T* out_re;
     T* out_im;
+    cx<T>* out_y;                      // C2R_HALVED: the caller's real array as pairs (bstride counts pairs)
+    int kmax;                          // R2C_DIRECT: the last row whose output index c + k out_rs is a stored bin (<= N/2)
     unsigned long long e0, de;
     __device__ __forceinline__ OddCol(const OddParams<T>& p, long long g) {
         const long long m = g / p.cols, c = g - m * p.cols;
@@ -1191,6 +1212,8 @@ struct OddCol {
         out_c = p.ws_out + m * p.n + c;
         out_re = p.out_re + m * p.bstride + c;
         out_im = p.out_im + m * p.bstride + c;
+        if constexpr (MODE == CHIRP_C2R_HALVED) out_y = reinterpret_cast<cx<T>*>(p.out_re) + m * p.bstride + c;
+        if constexpr (MODE == CHIRP_R2C_DIRECT) kmax = (int)((p.n / 2 - c) / p.out_rs);      // c < N / 3 on the last pass
     }
     // row r, times W_N^(e0 + r de)
     __device__ __forceinline__ cx<T> load(const OddParams<T>& p, int r) const {
@@ -1203,7 +1226,13 @@ struct OddCol {
     __device__ __forceinline__ void store(const OddParams<T>& p, int k, const cx<T>& v) const {
         if (p.role == ODD_A) {
             out_c[k * p.out_rs] = v;
+        } else if constexpr (MODE == CHIRP_C2R_HALVED) {
+            out_y[k * p.out_rs] = make_cx<T>(v.y * p.scale, v.x * p.scale);      // (y[2K], y[2K+1]) = swap(v) / L
+        } else if constexpr (MODE == CHIRP_C2R_DIRECT) {
+            out_re[k * p.out_rs] = v.y * p.scale;                               // the real part of the inverse, / N
         } else {
+            // R2C_DIRECT: the caller holds bins 0 .. floor(N/2) only
+            if (MODE == CHIRP_R2C_DIRECT && k > kmax) return;
             out_re[k * p.out_rs] = v.x * p.scale;
             out_im[k * p.out_rs] = v.y * p.scale;
         }
@@ -1211,12 +1240,12 @@ struct OddCol {
 };
 
 // R = RA * RB rows (RB = 1: one register DFT) held by one thread: no shared memory, a block covers ODD_NT adjacent columns.
-template <typename T, int RA, int RB>
-__global__ void __launch_bounds__(ODD_NT) odd_reg_kernel(const __grid_constant__ OddParams<T> p) {
+template <typename T, int RA, int RB, int MODE = CHIRP_C2C>
+__global__ void __launch_bounds__(ODD_NT, MODE == CHIRP_C2R_DIRECT ? 1 : 0) odd_reg_kernel(const __grid_constant__ OddParams<T> p) {
     constexpr int R = RA * RB;
     const long long g = (long long)blockIdx.x * ODD_NT + threadIdx.x;
     if (g >= p.total) return;
-    const OddCol<T> col(p, g);
+    const OddCol<T, MODE> col(p, g);
     cx<T> x[R];
 #pragma unroll
     for (int r = 0; r < R; ++r) x[r] = col.load(p, r);
@@ -1250,8 +1279,8 @@ __global__ void __launch_bounds__(ODD_NT) odd_reg_kernel(const __grid_constant__
 // One stage of the tile kernel over the butterflies row0, row0 + step, ...: FIRST reads the column's rows from global memory
 // (digit-reversed placement in the tile), LAST stores the output rows; the stages between work in place in shared memory.
 enum OddStage { ODD_FIRST, ODD_MID, ODD_LAST };
-template <typename T, int RAD, int STAGE>
-__device__ __forceinline__ void odd_tile_stage(const OddParams<T>& p, const OddCol<T>& col, cx<T>* sm, int L, int row0, int step,
+template <typename T, int RAD, int STAGE, int MODE>
+__device__ __forceinline__ void odd_tile_stage(const OddParams<T>& p, const OddCol<T, MODE>& col, cx<T>* sm, int L, int row0, int step,
                                                bool live) {
     const int nb = p.r / RAD;
     for (int b = row0; b < nb; b += step) {
@@ -1283,25 +1312,25 @@ __device__ __forceinline__ void odd_tile_stage(const OddParams<T>& p, const OddC
         }
     }
 }
-template <typename T, int STAGE>
-__device__ __forceinline__ void odd_tile_stage_of(int rad, const OddParams<T>& p, const OddCol<T>& col, cx<T>* sm, int L, int row0,
-                                                  int step, bool live) {
-    if (rad == 3) odd_tile_stage<T, 3, STAGE>(p, col, sm, L, row0, step, live);
-    else if (rad == 5) odd_tile_stage<T, 5, STAGE>(p, col, sm, L, row0, step, live);
-    else odd_tile_stage<T, 7, STAGE>(p, col, sm, L, row0, step, live);
+template <typename T, int STAGE, int MODE>
+__device__ __forceinline__ void odd_tile_stage_of(int rad, const OddParams<T>& p, const OddCol<T, MODE>& col, cx<T>* sm, int L,
+                                                  int row0, int step, bool live) {
+    if (rad == 3) odd_tile_stage<T, 3, STAGE, MODE>(p, col, sm, L, row0, step, live);
+    else if (rad == 5) odd_tile_stage<T, 5, STAGE, MODE>(p, col, sm, L, row0, step, live);
+    else odd_tile_stage<T, 7, STAGE, MODE>(p, col, sm, L, row0, step, live);
 }
 
 // R rows x cw adjacent columns in shared memory (cw * sizeof(cx<T>) >= 128 bytes, so the interleaved loads and the planar
 // stores both move in runs of 64 bytes or more), radix-3/5/7 stages between __syncthreads().  Thread t owns column t % cw
 // and every (ODD_NT / cw)-th butterfly of it.
-template <typename T>
+template <typename T, int MODE = CHIRP_C2C>
 __global__ void __launch_bounds__(ODD_NT, 2) odd_tile_kernel(const __grid_constant__ OddParams<T> p) {
     extern __shared__ __align__(16) unsigned char odd_smem[];
     const int c = threadIdx.x % p.cw, row0 = threadIdx.x / p.cw, step = ODD_NT / p.cw;
     cx<T>* sm = reinterpret_cast<cx<T>*>(odd_smem) + c;
     const long long g = (long long)blockIdx.x * p.cw + c;
     const bool live = g < p.total;
-    const OddCol<T> col(p, live ? g : p.total - 1);                    // a dead column computes its neighbour's and stores nothing
+    const OddCol<T, MODE> col(p, live ? g : p.total - 1);              // a dead column computes its neighbour's and stores nothing
     odd_tile_stage_of<T, ODD_FIRST>(p.rad[0], p, col, sm, 1, row0, step, live);
     int L = p.rad[0];
     for (int s = 1; s + 1 < p.nstages; ++s) {
@@ -1313,9 +1342,30 @@ __global__ void __launch_bounds__(ODD_NT, 2) odd_tile_kernel(const __grid_consta
     odd_tile_stage_of<T, ODD_LAST>(p.rad[p.nstages - 1], p, col, sm, L, row0, step, live);
 }
 
+// One ODD pass of r rows over `grid` blocks: the tile kernel when smem > 0, else the register kernel of r rows (false: none).
+template <typename T, int MODE>
+bool launch_odd_kernel(const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream) {
+    if (smem) {
+        odd_tile_kernel<T, MODE><<<grid, ODD_NT, smem, stream>>>(q);
+        return true;
+    }
+    switch (r) {
+        case 3: odd_reg_kernel<T, 3, 1, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 5: odd_reg_kernel<T, 5, 1, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 7: odd_reg_kernel<T, 7, 1, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 9: odd_reg_kernel<T, 3, 3, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 15: odd_reg_kernel<T, 5, 3, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 21: odd_reg_kernel<T, 7, 3, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 25: odd_reg_kernel<T, 5, 5, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        case 35: odd_reg_kernel<T, 7, 5, MODE><<<grid, ODD_NT, 0, stream>>>(q); return true;
+        default: return false;
+    }
+}
+
 // SMOOTH-PRE: ws[m N + n_o P + n_2] = (re, im)[m bstride + n_o + Q n_2].  A block transposes a tile of tq values of n_o by
 // tp values of n_2 through shared memory: it reads runs of tq adjacent elements and writes runs of tp adjacent complex values
-// (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).
+// (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).  The real modes load element n of z instead
+// (bstride is the input's member stride in T either way).
 constexpr int SMOOTH_TILE = 1024;
 template <typename T>
 struct SmoothParams {
@@ -1325,8 +1375,27 @@ struct SmoothParams {
     long long n, p, q, bstride;
     int tq, tp;
     unsigned tiles_q, tiles_per_member;
+    const cx<T>* wn_hi;            // C2R_HALVED: W_(2N)^e = wn_hi[e >> lo_bits] wn_lo[e & (2^lo_bits - 1)]
+    const cx<T>* wn_lo;
+    int lo_bits;
 };
+
+// W^e from a two-level table (hi[e >> lo_bits] lo[e & (2^lo_bits - 1)])
 template <typename T>
+__device__ __forceinline__ cx<T> two_level_root(const cx<T>* hi, const cx<T>* lo, int lo_bits, unsigned long long e) {
+    return cmul<T>(__ldg(hi + (e >> lo_bits)), __ldg(lo + (e & ((1ull << lo_bits) - 1))));
+}
+
+// SMOOTH-PRE's element n of a real mode's z, from the member's input re / im
+template <typename T, int MODE>
+__device__ __forceinline__ cx<T> smooth_real_in(const SmoothParams<T>& p, const T* re, const T* im, long long n) {
+    if constexpr (MODE == CHIRP_R2C_HALVED) return reinterpret_cast<const cx<T>*>(re)[n];     // (x[2n], x[2n+1]), pair-aligned
+    else if constexpr (MODE == CHIRP_R2C_DIRECT) return make_cx<T>(re[n], T(0));
+    else if constexpr (MODE == CHIRP_C2R_HALVED) return c2r_halved_in<T>(re, im, p.n, n, two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, n));
+    else return c2r_direct_in<T>(re, im, p.n, n);
+}
+
+template <typename T, int MODE = CHIRP_C2C>
 __global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__ SmoothParams<T> p) {
     __shared__ cx<T> sm[2 * SMOOTH_TILE];
     const unsigned m = blockIdx.x / p.tiles_per_member, tile = blockIdx.x - m * p.tiles_per_member;
@@ -1338,7 +1407,8 @@ __global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__
         const int j2 = i / p.tq, jo = i - j2 * p.tq;
         if (o + jo < p.q) {
             const long long src = o + jo + p.q * (a + j2);
-            sm[jo * pitch + j2] = make_cx<T>(re[src], im[src]);
+            if constexpr (MODE == CHIRP_C2C) sm[jo * pitch + j2] = make_cx<T>(re[src], im[src]);
+            else sm[jo * pitch + j2] = smooth_real_in<T, MODE>(p, re, im, src);
         }
     }
     __syncthreads();
@@ -1347,6 +1417,33 @@ __global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__
         const int jo = i / p.tp, j2 = i - jo * p.tp;
         if (o + jo < p.q) ws[(o + jo) * p.p + a + j2] = sm[jo * pitch + j2];
     }
+}
+
+// SMOOTH-POST-R2C, the halved r2c's untangle in place: the last ODD pass stored Z = DFT_L(z) in bins 0 .. L-1 of the caller's
+// arrays; the thread of pair (k, L - k), k <= L/2, replaces Z[k] and Z[L - k] with X[k] and X[L - k] (k = 0: X[0] and X[L];
+// L even: k = L/2 is the self pair).  A member-major grid of 256-thread blocks.
+template <typename T>
+struct SmoothPostParams {
+    T* re;
+    T* im;
+    const cx<T>* wn_hi;            // W_(2L) two-level, as SmoothParams
+    const cx<T>* wn_lo;
+    long long l, bstride;
+    int lo_bits;
+    unsigned blocks_per_member;
+};
+template <typename T>
+__global__ void __launch_bounds__(256) smooth_post_r2c_kernel(const __grid_constant__ SmoothPostParams<T> p) {
+    const unsigned mb = blockIdx.x / p.blocks_per_member;
+    const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * 256 + threadIdx.x;
+    if (2 * k > p.l) return;
+    T* re = p.re + (long long)mb * p.bstride;
+    T* im = p.im + (long long)mb * p.bstride;
+    const long long m = p.l - k, mm = k ? m : 0;
+    cx<T> xk, xm;
+    r2c_untangle<T>(make_cx<T>(re[k], im[k]), make_cx<T>(re[mm], im[mm]), two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, k), xk, xm);
+    re[k] = xk.x; im[k] = xk.y;
+    if (m != k) { re[m] = xm.x; im[m] = xm.y; }
 }
 
 }  // namespace phast

@@ -2371,10 +2371,11 @@ struct MixedSplit {
     int qa = 0, qb = 1;
 };
 
-// The split of n, or why it has none (`why` names the offending factor).
-bool mixed_split(size_t n, MixedSplit& out, std::string& why) {
-    if (n < 3 || is_pow2(n)) { why = "n = " + std::to_string(n) + " has no odd factor (powers of two take the c2c plan)"; return false; }
-    if (n > MIXED_MAX_N) { why = "n = " + std::to_string(n) + " is above 2^30 - 1"; return false; }
+// The split of n, or why it has none (`why` names the offending factor, and the length as `name`).
+bool mixed_split(size_t n, MixedSplit& out, std::string& why, const char* name = "n") {
+    const std::string nm = std::string(name) + " = " + std::to_string(n);
+    if (n < 3 || is_pow2(n)) { why = nm + " has no odd factor (powers of two take the c2c plan)"; return false; }
+    if (n > MIXED_MAX_N) { why = nm + " is above 2^30 - 1"; return false; }
     size_t p = 1, q = n;
     while (q % 2 == 0) { q /= 2; p *= 2; }
     size_t rest = q;
@@ -2384,7 +2385,7 @@ bool mixed_split(size_t n, MixedSplit& out, std::string& why) {
         size_t f = 11;
         while (f * f <= rest && rest % f) f += 2;
         if (rest % f) f = rest;
-        why = "n = " + std::to_string(n) + " has the prime factor " + std::to_string(f) + " (the mixed-radix path takes 2, 3, 5 and 7)";
+        why = nm + " has the prime factor " + std::to_string(f) + " (the mixed-radix path takes 2, 3, 5 and 7)";
         return false;
     }
     out.p = p;
@@ -2393,12 +2394,17 @@ bool mixed_split(size_t n, MixedSplit& out, std::string& why) {
     for (size_t a = 3; a * a <= q; a += 2)
         if (q % a == 0 && q / a <= (size_t)ODD_MAX_ROWS) best = a;
     if (!best) {
-        why = "n = " + std::to_string(n) + ": its odd part " + std::to_string(q) + " is not a product of two factors of at most " +
+        why = nm + ": its odd part " + std::to_string(q) + " is not a product of two factors of at most " +
               std::to_string(ODD_MAX_ROWS);
         return false;
     }
     out.qa = (int)best; out.qb = (int)(q / best);
     return true;
+}
+
+// "mixed 2^a x Q_a[ x Q_b]"
+std::string mixed_description(const MixedSplit& s) {
+    return "mixed 2^" + std::to_string(ilog2(s.p)) + " x " + std::to_string(s.qa) + (s.qb > 1 ? " x " + std::to_string(s.qb) : "");
 }
 
 // One ODD pass of R rows: the register kernel for one or two radices up to 35 rows (49 rows of f64 would spill), else the
@@ -2505,16 +2511,13 @@ int32_t build_mixed(Mixed<T>& mx, size_t n, const MixedSplit& split, int device)
     }
     CUDA_TRY(cudaFuncSetAttribute(odd_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   ODD_MAX_ROWS * 128));
+    CUDA_TRY(mixed_real_init<T>());
     return mx.w.init(n);                               // room for one member; batched calls grow it
 }
 
-template <typename T, int RA, int RB>
-void launch_odd_reg(const OddParams<T>& q, unsigned grid, cudaStream_t stream) {
-    odd_reg_kernel<T, RA, RB><<<grid, ODD_NT, 0, stream>>>(q);
-}
-
-// One ODD pass over `batch` members.  Launch record: R = rows, C = the columns a CTA covers.
-template <typename T>
+// One ODD pass over `batch` members, MODE the last pass's store (C2C for pass A).  Launch record: R = rows, C = the columns a
+// CTA covers; the kind carries -C2R / -R2C for the real stores.
+template <int MODE, typename T>
 int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cudaStream_t stream) {
     const OddPass<T>& ps = mx.pass[i];
     const size_t P = mx.split.p;
@@ -2531,39 +2534,64 @@ int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cuda
     const int cover = ps.cw ? ps.cw : ODD_NT;
     const size_t blocks = ((size_t)q.total + cover - 1) / cover;
     if (blocks > 0x7fffffffu) return fail(PHASTFT_ERR_INVALID_ARG, "batch * N is too large for one launch of the odd pass");
-    if (ps.cw) {
-        odd_tile_kernel<T><<<(unsigned)blocks, ODD_NT, (size_t)ps.r * ps.cw * sizeof(cx<T>), stream>>>(q);
-    } else {
-        switch (ps.r) {
-            case 3: launch_odd_reg<T, 3, 1>(q, (unsigned)blocks, stream); break;
-            case 5: launch_odd_reg<T, 5, 1>(q, (unsigned)blocks, stream); break;
-            case 7: launch_odd_reg<T, 7, 1>(q, (unsigned)blocks, stream); break;
-            case 9: launch_odd_reg<T, 3, 3>(q, (unsigned)blocks, stream); break;
-            case 15: launch_odd_reg<T, 5, 3>(q, (unsigned)blocks, stream); break;
-            case 21: launch_odd_reg<T, 7, 3>(q, (unsigned)blocks, stream); break;
-            case 25: launch_odd_reg<T, 5, 5>(q, (unsigned)blocks, stream); break;
-            case 35: launch_odd_reg<T, 7, 5>(q, (unsigned)blocks, stream); break;
-            default: return fail(PHASTFT_ERR_INVALID_ARG, "no register kernel of " + std::to_string(ps.r) + " rows");
-        }
-    }
+    const size_t smem = ps.cw ? (size_t)ps.r * ps.cw * sizeof(cx<T>) : 0;
+    const bool ok = MODE == CHIRP_C2C ? launch_odd_kernel<T, CHIRP_C2C>(q, ps.r, smem, (unsigned)blocks, stream)
+                                      : launch_odd_real<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream);
+    if (!ok) return fail(PHASTFT_ERR_INVALID_ARG, "no register kernel of " + std::to_string(ps.r) + " rows");
     CUDA_TRY(cudaGetLastError());
-    note_launch({"ODD", ps.r, 0, cover, ODD_NT, 0, ps.cw ? "tile" : "reg", false});
+    const char* name = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT ? "ODD-C2R" : MODE == CHIRP_R2C_DIRECT ? "ODD-R2C" : "ODD";
+    note_launch({name, ps.r, 0, cover, ODD_NT, 0, ps.cw ? "tile" : "reg", false});
     return PHASTFT_OK;
 }
 
-// One mixed-radix call of `batch` members: SMOOTH-PRE, the P-point plan on Q * batch workspace members, the ODD pass(es).
-// in / out are the caller's planar arrays, swapped for the reverse direction; scale is 1 or 1/N.
+// W_N^e for e < count from two tables of about sqrt(count) roots each: W_N^e = hi[e >> lo_bits] lo[e & (2^lo_bits - 1)]
+// (the real mixed plans' W_N, N = 2L, for the c2r pre-processing and the untangle)
 template <typename T>
-int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, T* out_re, T* out_im, size_t bstride, T scale, size_t batch,
-                  cudaStream_t stream) {
+struct TwoLevelRoots {
+    cx<T>* blob = nullptr;             // lo, then hi
+    const cx<T>* hi = nullptr;
+    const cx<T>* lo = nullptr;
+    int lo_bits = 0;
+};
+
+template <typename T>
+int32_t build_two_level(TwoLevelRoots<T>& t, size_t n, size_t count) {
+    int lc = 0;
+    while ((size_t(1) << lc) < count) ++lc;
+    t.lo_bits = (lc + 1) / 2;
+    const size_t n_lo = size_t(1) << t.lo_bits, n_hi = ((count - 1) >> t.lo_bits) + 1;
+    std::vector<cx<T>> v(n_lo + n_hi);
+    for (size_t j = 0; j < n_lo + n_hi; ++j) {
+        double re, im;
+        root_of_unity_any(j < n_lo ? j : (j - n_lo) << t.lo_bits, n, re, im);
+        v[j].x = (T)re; v[j].y = (T)im;
+    }
+    CUDA_TRY(cudaMalloc(&t.blob, v.size() * sizeof(cx<T>)));
+    CUDA_TRY(cudaMemcpy(t.blob, v.data(), v.size() * sizeof(cx<T>), cudaMemcpyHostToDevice));
+    t.lo = t.blob; t.hi = t.blob + n_lo;
+    return PHASTFT_OK;
+}
+
+// One mixed-radix call of `batch` members: SMOOTH-PRE, the P-point plan on Q * batch workspace members, the ODD pass(es), with
+// the ends in MODE (CHIRP_C2C for the complex plan; the real modes as in CHIRP-PRE / CHIRP-POST, fft_kernels.cuh).  in / out
+// are the caller's arrays, swapped for the reverse direction; in_bstride counts T, out_bstride what the last pass stores (T,
+// or pairs for C2R_HALVED); scale is 1, 1/N or 1/L.  `wn` is the real plan's W_(2L) for the halved modes.  The halved r2c ends
+// with SMOOTH-POST-R2C on the bins.  The workspace follows AnyWorkspace's protocol (`reserve_fn` names the call that grows it).
+template <int MODE, typename T>
+int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_bstride, T* out_re, T* out_im, size_t out_bstride,
+                  T scale, size_t batch, cudaStream_t stream, const char* reserve_fn, const TwoLevelRoots<T>* wn = nullptr) {
+    constexpr bool r2c = MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT, c2r = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT;
+    constexpr int LAST = MODE == CHIRP_R2C_HALVED ? CHIRP_C2C : MODE;   // the halved r2c stores Z, then untangles it in place
     DeviceGuard g(mx.device);
     const size_t P = mx.split.p, Q = (size_t)mx.split.qa * mx.split.qb;
     std::lock_guard<std::mutex> lock(mx.w.mu);
     bool capturing = false;
-    if (int32_t st = mx.w.acquire(batch * mx.n, batch, stream, "phastft_plan_any_*_reserve", capturing)) return st;
+    if (int32_t st = mx.w.acquire(batch * mx.n, batch, stream, reserve_fn, capturing)) return st;
     SmoothParams<T> sp;
+    memset(&sp, 0, sizeof(sp));
     sp.in_re = in_re; sp.in_im = in_im; sp.ws = mx.w.ws;
-    sp.n = (long long)mx.n; sp.p = (long long)P; sp.q = (long long)Q; sp.bstride = (long long)bstride;
+    sp.n = (long long)mx.n; sp.p = (long long)P; sp.q = (long long)Q; sp.bstride = (long long)in_bstride;
+    if (wn) { sp.wn_hi = wn->hi; sp.wn_lo = wn->lo; sp.lo_bits = wn->lo_bits; }
     // runs as long as Q and P allow within SMOOTH_TILE values: up to 32 values of n_o, then n_2, then the rest of n_o when P is short
     size_t tq = std::min<size_t>(Q, 32), tq2 = 1;
     while (tq2 < tq) tq2 *= 2;
@@ -2576,10 +2604,12 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, T* out_re,
     for (size_t done = 0; done < batch; done += max_members) {
         const size_t nb = std::min(batch - done, max_members);
         SmoothParams<T> s2 = sp;
-        s2.in_re += done * bstride; s2.in_im += done * bstride; s2.ws += done * mx.n;
-        smooth_pre_kernel<T><<<(unsigned)(nb * sp.tiles_per_member), 256, 0, stream>>>(s2);
+        s2.in_re += done * in_bstride; s2.ws += done * mx.n;
+        if (s2.in_im) s2.in_im += done * in_bstride;
+        if constexpr (MODE == CHIRP_C2C) smooth_pre_kernel<T><<<(unsigned)(nb * sp.tiles_per_member), 256, 0, stream>>>(s2);
+        else launch_smooth_pre_real<T>(MODE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
         CUDA_TRY(cudaGetLastError());
-        note_launch({"SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0, "plain", false});
+        note_launch({r2c ? "SMOOTH-PRE-R2C" : c2r ? "SMOOTH-PRE-C2R" : "SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0, "plain", false});
     }
     if (P > 1) {
         Io<T> io;
@@ -2593,9 +2623,27 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, T* out_re,
     memset(&q, 0, sizeof(q));
     q.ws = mx.w.ws; q.ws_out = mx.w.ws; q.out_re = out_re; q.out_im = out_im;
     q.wn_hi = mx.wn_hi; q.wn_lo = mx.wn_lo; q.lo_bits = mx.lo_bits;
-    q.n = (long long)mx.n; q.p = (long long)P; q.bstride = (long long)bstride; q.scale = scale;
+    q.n = (long long)mx.n; q.p = (long long)P; q.bstride = (long long)out_bstride; q.scale = scale;
     for (int i = 0; i < mx.npasses; ++i)
-        if (int32_t st = launch_odd(mx, i, q, batch, stream)) return st;
+        if (int32_t st = i + 1 < mx.npasses ? launch_odd<CHIRP_C2C>(mx, i, q, batch, stream) : launch_odd<LAST>(mx, i, q, batch, stream))
+            return st;
+    if constexpr (MODE == CHIRP_R2C_HALVED) {
+        // Launch record: R = L, C = the members of that launch
+        SmoothPostParams<T> pp;
+        pp.re = out_re; pp.im = out_im; pp.wn_hi = wn->hi; pp.wn_lo = wn->lo; pp.lo_bits = wn->lo_bits;
+        pp.l = (long long)mx.n; pp.bstride = (long long)out_bstride;
+        const size_t bpm = (mx.n / 2 + 1 + 255) / 256;
+        pp.blocks_per_member = (unsigned)bpm;
+        const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+        for (size_t done = 0; done < batch; done += max_members) {
+            const size_t nb = std::min(batch - done, max_members);
+            SmoothPostParams<T> p2 = pp;
+            p2.re += done * out_bstride; p2.im += done * out_bstride;
+            launch_smooth_post_r2c<T>(p2, (unsigned)(nb * bpm), stream);
+            CUDA_TRY(cudaGetLastError());
+            note_launch({"SMOOTH-POST-R2C", (int)mx.n, 0, (int)nb, 256, 0, "plain", false});
+        }
+    }
     return mx.w.release(stream, capturing);
 }
 
@@ -2747,9 +2795,7 @@ int32_t build_plan_any(size_t n, int device, int algo, PlanAny<T>** out) {
     }
     if (mixed) {
         if (int32_t st = build_mixed(pl->mx, n, split, device)) return st;
-        pl->description = "n=" + std::to_string(n) + prec + " any: mixed 2^" + std::to_string(ilog2(split.p)) + " x " +
-                          std::to_string(split.qa) + (split.qb > 1 ? " x " + std::to_string(split.qb) : "") + " | inner: " +
-                          pl->mx.inner->description;
+        pl->description = "n=" + std::to_string(n) + prec + " any: " + mixed_description(split) + " | inner: " + pl->mx.inner->description;
         *out = pl.release();
         return PHASTFT_OK;
     }
@@ -2844,8 +2890,8 @@ int32_t any_dev(const PlanAny<T>* pl, T* d_re, T* d_im, int direction, size_t ba
     // the reverse direction by the swap trick (fft_dev): re and im exchanged on the way in and out, 1/N folded into CHIRP-POST
     const bool fwd = direction == PHASTFT_FORWARD;
     if (pl->mx.inner)
-        return mixed_run(pl->mx, fwd ? d_re : d_im, fwd ? d_im : d_re, fwd ? d_re : d_im, fwd ? d_im : d_re, bstride,
-                         fwd ? T(1) : T(1) / (T)pl->n, batch, stream);
+        return mixed_run<CHIRP_C2C>(pl->mx, fwd ? d_re : d_im, fwd ? d_im : d_re, bstride, fwd ? d_re : d_im, fwd ? d_im : d_re, bstride,
+                                    fwd ? T(1) : T(1) / (T)pl->n, batch, stream, "phastft_plan_any_*_reserve");
     ChirpParams<T> cp;
     memset(&cp, 0, sizeof(cp));
     cp.in_re = cp.out_re = fwd ? d_re : d_im;
@@ -2891,20 +2937,25 @@ int32_t any_host(const PlanAny<T>* pl, T* re, size_t len_re, T* im, size_t len_i
 }
 
 // =================================================================================================
-// real input of any length: r2c / c2r over Bluestein (the CHIRP-*-R2C / -C2R kernel modes)
+// real input of any length: r2c / c2r over Bluestein (the CHIRP-*-R2C / -C2R kernel modes) or the mixed-radix path (the same
+// modes of SMOOTH-PRE and the last ODD pass, and SMOOTH-POST-R2C)
 // =================================================================================================
 // Even N up to 2^30 - 2 take the halved path (Bluestein of L = N/2, M <= 2^30); odd N the direct one (L = N, up to 2^29 - 1);
-// powers of two from 4 the r2c plan.
+// powers of two from 4 the r2c plan.  On the mixed path even N go up to 2^31 - 2 (L = N/2 <= 2^30 - 1).
 constexpr size_t R2C_ANY_MAX_EVEN = (size_t(1) << 30) - 2;
 
 template <typename T>
 struct PlanR2cAny {
     size_t n = 0;
     int device = 0;
-    bool halved = false;               // even N: Bluestein of L = N/2 over z[m] = x[2m] + i x[2m+1]; odd N: L = N
+    bool halved = false;               // even N: the L-point transform of z[m] = x[2m] + i x[2m+1], L = N/2; odd N: L = N
     PlanR2c<T>* pow2 = nullptr;        // N a power of two >= 4: the r2c plan, run as it is
-    Bluestein<T> bs;
-    cx<T>* wn = nullptr;               // halved: W_N^k for k = 0 .. floor(L/2), rounded to T
+    Bluestein<T> bs;                   // otherwise: Bluestein of L ...
+    Mixed<T> mx;                       // ... or the mixed-radix path of L (mx.inner set)
+    cx<T>* wn = nullptr;               // halved Bluestein: W_N^k for k = 0 .. floor(L/2), rounded to T
+    TwoLevelRoots<T> wn2;              // halved mixed: W_N^e for e < L, two-level
+    AnyWorkspace<T>& workspace() const { return mx.inner ? mx.w : bs.w; }
+    cudaStream_t host_stream() const { return (mx.inner ? mx.inner : bs.inner)->stream; }
     mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then the workspace's mu)
     mutable T* stage_real = nullptr;   // host-API staging: N reals, floor(N/2) + 1 bins
     mutable T* stage_re = nullptr;
@@ -2912,23 +2963,31 @@ struct PlanR2cAny {
     std::string description;
     ~PlanR2cAny() {
         DeviceGuard g(device);
-        for (void* p : {(void*)wn, (void*)stage_real, (void*)stage_re, (void*)stage_im})
+        for (void* p : {(void*)wn, (void*)wn2.blob, (void*)stage_real, (void*)stage_re, (void*)stage_im})
             if (p) cudaFree(p);
         delete pow2;
     }
 };
 
 template <typename T>
-int32_t build_plan_r2c_any(size_t n, int device, PlanR2cAny<T>** out) {
+int32_t build_plan_r2c_any(size_t n, int device, int algo, PlanR2cAny<T>** out) {
     if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
     *out = nullptr;
     if (n == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n must be >= 1");
+    if (algo != PHASTFT_ANY_BLUESTEIN && algo != PHASTFT_ANY_MIXED && algo != PHASTFT_ANY_AUTO)
+        return fail(PHASTFT_ERR_INVALID_ARG, "algo must be PHASTFT_ANY_BLUESTEIN, PHASTFT_ANY_MIXED or PHASTFT_ANY_AUTO");
     const bool pow2 = n >= 4 && is_pow2(n);
     if (pow2 && n > (size_t(1) << 31)) return fail(PHASTFT_ERR_INVALID_ARG, "n = " + std::to_string(n) + " is a power of two above 2^31");
-    if (!pow2 && n % 2 == 0 && n > R2C_ANY_MAX_EVEN)
+    // the mixed path runs on L = N/2 (halved) or N (direct) when that length is eligible
+    const size_t l = n % 2 == 0 ? n / 2 : n;
+    MixedSplit split;
+    std::string why;
+    const bool mixed = !pow2 && algo != PHASTFT_ANY_BLUESTEIN && mixed_split(l, split, why, n % 2 == 0 ? "L = n/2" : "n");
+    if (!pow2 && algo == PHASTFT_ANY_MIXED && !mixed) return fail(PHASTFT_ERR_INVALID_ARG, "no mixed-radix plan: " + why);
+    if (!pow2 && !mixed && n % 2 == 0 && n > R2C_ANY_MAX_EVEN)
         return fail(PHASTFT_ERR_INVALID_ARG, "even n = " + std::to_string(n) + " above 2^30 - 2 (its half-length convolution would "
                                              "exceed 2^30 points)");
-    if (n % 2 && n > ANY_MAX_N)
+    if (!mixed && n % 2 && n > ANY_MAX_N)
         return fail(PHASTFT_ERR_INVALID_ARG, "odd n = " + std::to_string(n) + " above 2^29 - 1 (its convolution would exceed 2^30 points)");
     std::unique_ptr<PlanR2cAny<T>> pl(new PlanR2cAny<T>());
     pl->n = n; pl->device = device;
@@ -2941,7 +3000,17 @@ int32_t build_plan_r2c_any(size_t n, int device, PlanR2cAny<T>** out) {
         return PHASTFT_OK;
     }
     pl->halved = n % 2 == 0;
-    const size_t l = pl->halved ? n / 2 : n;
+    if (mixed) {
+        if (int32_t st = build_mixed(pl->mx, l, split, device)) return st;
+        if (pl->halved) {
+            DeviceGuard g(device);
+            if (int32_t st = build_two_level(pl->wn2, n, l)) return st;
+        }
+        pl->description = head + (pl->halved ? "halved, " : "direct, ") + mixed_description(split) + " | inner: " +
+                          pl->mx.inner->description;
+        *out = pl.release();
+        return PHASTFT_OK;
+    }
     if (int32_t st = build_bluestein(pl->bs, l, device)) return st;
     if (pl->halved) {
         // W_N^k = exp(-2 pi i k / N) by exact integer reduction in long double, rounded to T, for the k <= L/2 the kernels read
@@ -2985,13 +3054,18 @@ int32_t r2c_any_dev(const PlanR2cAny<T>* pl, const T* d_in, size_t in_stride, T*
         if (int32_t st = check_pair_alignment(d_in, "d_input")) return st;
     }
     if (batch == 0) return PHASTFT_OK;
+    const char* res = "phastft_plan_r2c_any_*_reserve";
+    if (pl->mx.inner)
+        return pl->halved ? mixed_run<CHIRP_R2C_HALVED, T>(pl->mx, d_in, nullptr, in_stride, d_ore, d_oim, out_stride, T(1), batch, stream,
+                                                        res, &pl->wn2)
+                          : mixed_run<CHIRP_R2C_DIRECT, T>(pl->mx, d_in, nullptr, in_stride, d_ore, d_oim, out_stride, T(1), batch, stream,
+                                                        res);
     ChirpParams<T> cp;
     memset(&cp, 0, sizeof(cp));
     cp.in_re = d_in; cp.out_re = d_ore; cp.out_im = d_oim;
     cp.bstride = (long long)in_stride; cp.out_bstride = (long long)out_stride;
     cp.scale = T(1);
     cp.wn = pl->wn;
-    const char* res = "phastft_plan_r2c_any_*_reserve";
     return pl->halved ? bluestein_run<CHIRP_R2C_HALVED>(pl->bs, cp, batch, stream, res)
                       : bluestein_run<CHIRP_R2C_DIRECT>(pl->bs, cp, batch, stream, res);
 }
@@ -3015,13 +3089,21 @@ int32_t c2r_any_dev(const PlanR2cAny<T>* pl, const T* d_ire, const T* d_iim, siz
         if (int32_t st = check_pair_alignment(d_out, "d_output")) return st;
     }
     if (batch == 0) return PHASTFT_OK;
+    const char* res = "phastft_plan_r2c_any_*_reserve";
+    if (pl->mx.inner) {
+        const T scale = T(1) / (T)pl->mx.n;
+        // the halved c2r stores the pairs (y[2k], y[2k+1]): its member stride counts pairs
+        return pl->halved ? mixed_run<CHIRP_C2R_HALVED, T>(pl->mx, d_ire, d_iim, in_stride, d_out, nullptr, out_stride / 2, scale, batch,
+                                                        stream, res, &pl->wn2)
+                          : mixed_run<CHIRP_C2R_DIRECT, T>(pl->mx, d_ire, d_iim, in_stride, d_out, nullptr, out_stride, scale, batch,
+                                                        stream, res);
+    }
     ChirpParams<T> cp;
     memset(&cp, 0, sizeof(cp));
     cp.in_re = d_ire; cp.in_im = d_iim; cp.out_re = d_out;
     cp.bstride = (long long)in_stride; cp.out_bstride = (long long)out_stride;
     cp.scale = T(1) / (T)pl->bs.l;
     cp.wn = pl->wn;
-    const char* res = "phastft_plan_r2c_any_*_reserve";
     return pl->halved ? bluestein_run<CHIRP_C2R_HALVED>(pl->bs, cp, batch, stream, res)
                       : bluestein_run<CHIRP_C2R_DIRECT>(pl->bs, cp, batch, stream, res);
 }
@@ -3030,13 +3112,14 @@ template <typename T>
 int32_t r2c_any_reserve(const PlanR2cAny<T>* pl, size_t batch) {
     if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
     if (pl->pow2) return r2c_reserve(pl->pow2, batch);
+    if (pl->mx.inner) return mixed_reserve(pl->mx, batch);
     return bluestein_reserve(pl->bs, batch);
 }
 
 // Caller holds host_mu.
 template <typename T>
 int32_t ensure_r2c_any_staging(const PlanR2cAny<T>* pl) {
-    std::lock_guard<std::mutex> lock(pl->bs.w.mu);       // released before the device call, which takes it
+    std::lock_guard<std::mutex> lock(pl->workspace().mu);   // released before the device call, which takes it
     if (!pl->stage_real) CUDA_TRY(cudaMalloc(&pl->stage_real, pl->n * sizeof(T)));
     if (!pl->stage_re) CUDA_TRY(cudaMalloc(&pl->stage_re, (pl->n / 2 + 1) * sizeof(T)));
     if (!pl->stage_im) CUDA_TRY(cudaMalloc(&pl->stage_im, (pl->n / 2 + 1) * sizeof(T)));
@@ -3056,7 +3139,7 @@ int32_t r2c_any_host(const PlanR2cAny<T>* pl, const T* in, size_t len_in, T* ore
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> host_lock(pl->host_mu);
     if (int32_t st = ensure_r2c_any_staging(pl)) return st;
-    cudaStream_t s = pl->bs.inner->stream;
+    cudaStream_t s = pl->host_stream();
     CUDA_TRY(cudaMemcpyAsync(pl->stage_real, in, n * sizeof(T), cudaMemcpyHostToDevice, s));
     if (int32_t st = r2c_any_dev(pl, pl->stage_real, n, pl->stage_re, pl->stage_im, bins, 1, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(ore, pl->stage_re, bins * sizeof(T), cudaMemcpyDeviceToHost, s));
@@ -3077,7 +3160,7 @@ int32_t c2r_any_host(const PlanR2cAny<T>* pl, const T* ire, size_t len_ire, cons
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> host_lock(pl->host_mu);
     if (int32_t st = ensure_r2c_any_staging(pl)) return st;
-    cudaStream_t s = pl->bs.inner->stream;
+    cudaStream_t s = pl->host_stream();
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, ire, bins * sizeof(T), cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_im, iim, bins * sizeof(T), cudaMemcpyHostToDevice, s));
     if (int32_t st = c2r_any_dev(pl, pl->stage_re, pl->stage_im, bins, pl->stage_real, n, 1, s)) return st;
@@ -3356,7 +3439,14 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
     }                                                                                                                   \
     int32_t phastft_plan_r2c_any_##SFX##_create(size_t n, int device, phastft_plan_r2c_any_##SFX** out) {               \
         PlanR2cAny<T>* pl = nullptr;                                                                                    \
-        int32_t st = build_plan_r2c_any<T>(n, device, &pl);                                                             \
+        int32_t st = build_plan_r2c_any<T>(n, device, PHASTFT_ANY_BLUESTEIN, &pl);                                      \
+        if (out) *out = reinterpret_cast<phastft_plan_r2c_any_##SFX*>(pl);                                              \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    int32_t phastft_plan_r2c_any_##SFX##_create_with(size_t n, int device, int algo, phastft_plan_r2c_any_##SFX** out) {\
+        PlanR2cAny<T>* pl = nullptr;                                                                                    \
+        int32_t st = build_plan_r2c_any<T>(n, device, algo, &pl);                                                       \
         if (out) *out = reinterpret_cast<phastft_plan_r2c_any_##SFX*>(pl);                                              \
         else if (pl) delete pl;                                                                                         \
         return st;                                                                                                      \

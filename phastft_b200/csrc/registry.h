@@ -2,7 +2,8 @@
 //
 // The kernels are instantiated in several translation units so the library builds in parallel
 // (__graft_entry__.build()): reg_strided.cu (COL / TRANS passes, compiled once per precision and kind),
-// reg_row.cu (whole-transform-in-one-CTA kernels), reg_multi.cu (cluster and pipelined two-pass launches).
+// reg_row.cu (whole-transform-in-one-CTA kernels), reg_multi.cu (cluster and pipelined two-pass launches), mixed_real.cu (the
+// real modes of the mixed-radix kernels).
 // phastft_cuda.cu holds the planner, the launcher and the C ABI and only sees these descriptors.
 #pragma once
 #include <string>
@@ -119,5 +120,12 @@ template <typename T> void add_row_kernels(std::vector<KernelEntry<T>>& v);
 template <typename T, int KIND> void add_strided_kernels(std::vector<KernelEntry<T>>& v);
 template <typename T> const std::vector<PipeEntry<T>>& pipe_registry();
 template <typename T> const std::vector<ClusterEntry<T>>& cluster_registry();
+
+// defined in mixed_real.cu: the launches of the real any-length plan's mixed-radix kernels (the ChirpMode `mode` of SMOOTH-PRE
+// and of the last ODD pass, launch_odd_kernel's arguments), and the tile kernels' shared-memory limit
+template <typename T> cudaError_t mixed_real_init();
+template <typename T> bool launch_odd_real(int mode, const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_smooth_pre_real(int mode, const SmoothParams<T>& p, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_smooth_post_r2c(const SmoothPostParams<T>& p, unsigned grid, cudaStream_t stream);
 
 }  // namespace phast

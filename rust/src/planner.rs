@@ -156,10 +156,10 @@ impl_planner_any!(PlannerAny32, ffi::phastft_plan_any_f32, phastft_plan_any_f32_
                   phastft_plan_any_f32_size, phastft_plan_any_f32_describe, phastft_plan_any_f32_reserve);
 
 macro_rules! impl_planner_r2c_any {
-    ($name:ident, $raw:ty, $create:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
+    ($name:ident, $raw:ty, $create:ident, $create_with:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
         /// Additive (the reference's r2c accepts powers of two >= 4 only): real-input FFTs of any length.  A power of two
         /// from 4 runs the r2c plan as it is; an even length up to 2^30 - 2 runs Bluestein's algorithm on N/2 complex
-        /// points, an odd one up to 2^29 - 1 on N.
+        /// points, an odd one up to 2^29 - 1 on N.  `with_algo` selects the mixed-radix path of N/2 or N instead.
         pub struct $name {
             pub(crate) raw: *mut $raw,
         }
@@ -172,12 +172,19 @@ macro_rules! impl_planner_r2c_any {
                 check(unsafe { ffi::$create(n, device(), &mut raw) });
                 Self { raw }
             }
+            /// `new` with the algorithm chosen (`Mixed` / `Auto`: the mixed-radix path of N/2 for even N up to 2^31 - 2, of N for
+            /// odd N, when that length is eligible).  Panics as `new` does, and for `AnyAlgo::Mixed` on a length that is not eligible.
+            pub fn with_algo(n: usize, algo: AnyAlgo) -> Self {
+                let mut raw = std::ptr::null_mut();
+                check(unsafe { ffi::$create_with(n, device(), algo as std::os::raw::c_int, &mut raw) });
+                Self { raw }
+            }
             /// Number of real points the planner was built for.
             pub fn n(&self) -> usize {
                 unsafe { ffi::$size(self.raw) }
             }
-            /// `"n=44100 f64 r2c any: halved, Bluestein L=22050 M=2^16 | inner: ..."`, `"... direct, ..."` or
-            /// `"n=2^20 f64 r2c any: power of two | ..."`.
+            /// `"n=44100 f64 r2c any: halved, Bluestein L=22050 M=2^16 | inner: ..."`, `"... halved, mixed 2^1 x 105 x 105 | ..."`,
+            /// `"... direct, ..."` or `"n=2^20 f64 r2c any: power of two | ..."`.
             pub fn describe(&self) -> String {
                 unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
             }
@@ -193,7 +200,9 @@ macro_rules! impl_planner_r2c_any {
         }
     };
 }
-impl_planner_r2c_any!(PlannerR2cAny64, ffi::phastft_plan_r2c_any_f64, phastft_plan_r2c_any_f64_create, phastft_plan_r2c_any_f64_destroy,
+impl_planner_r2c_any!(PlannerR2cAny64, ffi::phastft_plan_r2c_any_f64, phastft_plan_r2c_any_f64_create,
+                      phastft_plan_r2c_any_f64_create_with, phastft_plan_r2c_any_f64_destroy,
                       phastft_plan_r2c_any_f64_size, phastft_plan_r2c_any_f64_describe, phastft_plan_r2c_any_f64_reserve);
-impl_planner_r2c_any!(PlannerR2cAny32, ffi::phastft_plan_r2c_any_f32, phastft_plan_r2c_any_f32_create, phastft_plan_r2c_any_f32_destroy,
+impl_planner_r2c_any!(PlannerR2cAny32, ffi::phastft_plan_r2c_any_f32, phastft_plan_r2c_any_f32_create,
+                      phastft_plan_r2c_any_f32_create_with, phastft_plan_r2c_any_f32_destroy,
                       phastft_plan_r2c_any_f32_size, phastft_plan_r2c_any_f32_describe, phastft_plan_r2c_any_f32_reserve);
