@@ -7,6 +7,7 @@
 // what() is the reference's panic message.  Header-only; link with -lphastft_cuda.
 #pragma once
 
+#include <complex>
 #include <cstddef>
 #include <stdexcept>
 #include <string>
@@ -77,6 +78,8 @@ template <> struct Api<double> {
     static int32_t any_reserve(const Any* p, std::size_t b) { return phastft_plan_any_f64_reserve(p, b); }
     static int32_t any_dev(const Any* p, double* re, double* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f64_dev(p, re, im, d, b, st, s); }
     static int32_t any_host(const Any* p, double* re, std::size_t lr, double* im, std::size_t li, int d) { return phastft_fft_any_f64_host(p, re, lr, im, li, d); }
+    static int32_t any_il_dev(const Any* p, double* sig, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_interleaved_any_f64_dev(p, sig, d, b, st, s); }
+    static int32_t any_il_host(const Any* p, double* sig, std::size_t len, int d) { return phastft_fft_interleaved_any_f64_host(p, sig, len, d); }
     using R2cAny = phastft_plan_r2c_any_f64;
     static int32_t r2c_any_create(std::size_t n, int dev, int algo, R2cAny** o) { return phastft_plan_r2c_any_f64_create_with(n, dev, algo, o); }
     static void r2c_any_destroy(R2cAny* p) { phastft_plan_r2c_any_f64_destroy(p); }
@@ -116,6 +119,8 @@ template <> struct Api<float> {
     static int32_t any_reserve(const Any* p, std::size_t b) { return phastft_plan_any_f32_reserve(p, b); }
     static int32_t any_dev(const Any* p, float* re, float* im, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_any_f32_dev(p, re, im, d, b, st, s); }
     static int32_t any_host(const Any* p, float* re, std::size_t lr, float* im, std::size_t li, int d) { return phastft_fft_any_f32_host(p, re, lr, im, li, d); }
+    static int32_t any_il_dev(const Any* p, float* sig, int d, std::size_t b, std::size_t st, void* s) { return phastft_fft_interleaved_any_f32_dev(p, sig, d, b, st, s); }
+    static int32_t any_il_host(const Any* p, float* sig, std::size_t len, int d) { return phastft_fft_interleaved_any_f32_host(p, sig, len, d); }
     using R2cAny = phastft_plan_r2c_any_f32;
     static int32_t r2c_any_create(std::size_t n, int dev, int algo, R2cAny** o) { return phastft_plan_r2c_any_f32_create_with(n, dev, algo, o); }
     static void r2c_any_destroy(R2cAny* p) { phastft_plan_r2c_any_f32_destroy(p); }
@@ -206,6 +211,15 @@ class PlannerAny {
     /// `batch` transforms on device pointers, transform b at b * batch_stride; stream-ordered on `stream`
     void fft_device(T* d_reals, T* d_imags, Direction d, std::size_t batch, std::size_t batch_stride, void* stream = nullptr) const {
         check(Api<T>::any_dev(raw_, d_reals, d_imags, (int)d, batch, batch_stride, stream));
+    }
+    /// in place on `len` interleaved host values (len == N, else the length panic); the same results as fft()
+    void fft_interleaved(std::complex<T>* signal, std::size_t len, Direction d) const {
+        check(Api<T>::any_il_host(raw_, reinterpret_cast<T*>(signal), len, (int)d));
+    }
+    /// `batch` transforms on an interleaved device array, transform b at complex element b * batch_stride
+    void fft_interleaved_device(std::complex<T>* d_signal, Direction d, std::size_t batch, std::size_t batch_stride,
+                                void* stream = nullptr) const {
+        check(Api<T>::any_il_dev(raw_, reinterpret_cast<T*>(d_signal), (int)d, batch, batch_stride, stream));
     }
   private:
     typename Api<T>::Any* raw_ = nullptr;

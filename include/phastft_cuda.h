@@ -50,8 +50,9 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * CHIRP-POST-R2C / CHIRP-PRE-C2R / CHIRP-POST-C2R (the same around the real any-length transforms), SMOOTH-PRE (the mixed-radix
  * path's de-interleave: R=<P>, C=<workspace members>) and ODD (its radix-3/5/7 passes: R=<rows>, C=<columns per CTA>, mode reg
  * for the register kernel or tile for the shared-memory one), SMOOTH-PRE-R2C / SMOOTH-PRE-C2R and ODD-R2C / ODD-C2R (the same with
- * the real any-length transforms' loads and last-pass stores) and SMOOTH-POST-R2C (their halved r2c's untangle: R=<L>,
- * C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * the real any-length transforms' loads and last-pass stores), SMOOTH-POST-R2C (their halved r2c's untangle: R=<L>,
+ * C=<members>) and CHIRP-PRE-IL / CHIRP-POST-IL / SMOOTH-PRE-IL / ODD-IL (the complex any-length transform's end kernels, the
+ * last ODD pass only, in phastft_fft_interleaved_any_*: R, C and NT as in the planar call); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
@@ -324,6 +325,23 @@ PHASTFT_API int32_t phastft_fft_any_f64_host(const phastft_plan_any_f64* plan, d
                                              size_t len_im, int direction);
 PHASTFT_API int32_t phastft_fft_any_f32_host(const phastft_plan_any_f32* plan, float* reals, size_t len_re, float* imags,
                                              size_t len_im, int direction);
+/* The same transforms on interleaved (re, im) pairs (torch.complex128 / complex64, std::complex<T>, num_complex::Complex<T>),
+ * with any plan phastft_plan_any_*_create or _create_with built: member b starts at complex element b * batch_stride_complex
+ * (>= n when batch > 1), in place, natural order, forward unscaled, reverse scaled by 1/n.  d_signal must be aligned to
+ * 2 * sizeof(T) bytes.  Powers of two run phastft_fft_interleaved_*_dev on the plan's n-point plan; Bluestein and mixed-radix
+ * plans run the kernels of phastft_fft_any_*_dev with the interleaved layout at both ends (CHIRP-PRE-IL / CHIRP-POST-IL,
+ * SMOOTH-PRE-IL / ODD-IL) and give the planar call's results bit for bit.  Workspace, reserve() and batch == 0 as in
+ * phastft_fft_any_*_dev; NULL or misaligned pointers, bad directions and short strides return PHASTFT_ERR_INVALID_ARG before any
+ * launch.  The host form stages through a buffer of n complex values that its first call allocates; len_complex != n returns
+ * PHASTFT_ERR_PLAN_MISMATCH. */
+PHASTFT_API int32_t phastft_fft_interleaved_any_f64_dev(const phastft_plan_any_f64* plan, double* d_signal, int direction,
+                                                        size_t batch, size_t batch_stride_complex, void* stream);
+PHASTFT_API int32_t phastft_fft_interleaved_any_f32_dev(const phastft_plan_any_f32* plan, float* d_signal, int direction,
+                                                        size_t batch, size_t batch_stride_complex, void* stream);
+PHASTFT_API int32_t phastft_fft_interleaved_any_f64_host(const phastft_plan_any_f64* plan, double* signal, size_t len_complex,
+                                                         int direction);
+PHASTFT_API int32_t phastft_fft_interleaved_any_f32_host(const phastft_plan_any_f32* plan, float* signal, size_t len_complex,
+                                                         int direction);
 
 /* ---- real-input FFTs of any length (the reference's r2c / c2r accept powers of two >= 4 only) ---------------------------
  * r2c reads n reals and writes the n/2 + 1 bins X[0 .. floor(n/2)], planar, forward, unscaled.  c2r reads n/2 + 1 bins and

@@ -114,6 +114,8 @@ SIGNATURES = {
     "phastft_plan_any_{s}_reserve": ([_vp, _sz], _i32),
     "phastft_fft_any_{s}_dev": ([_vp, _vp, _vp, _ci, _sz, _sz, _vp], _i32),
     "phastft_fft_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _ci], _i32),
+    "phastft_fft_interleaved_any_{s}_dev": ([_vp, _vp, _ci, _sz, _sz, _vp], _i32),
+    "phastft_fft_interleaved_any_{s}_host": ([_vp, _vp, _sz, _ci], _i32),
     "phastft_plan_r2c_any_{s}_create": ([_sz, _ci, C.POINTER(_vp)], _i32),
     "phastft_plan_r2c_any_{s}_create_with": ([_sz, _ci, _ci, C.POINTER(_vp)], _i32),
     "phastft_plan_r2c_any_{s}_destroy": ([_vp], None),

@@ -42,6 +42,7 @@ __all__ = [
     "AnyAlgo", "PlannerAny64", "PlannerAny32", "fft_64_any_with_planner", "fft_32_any_with_planner", "fft_any_batch",
     "PlannerR2cAny64", "PlannerR2cAny32", "r2c_fft_f64_any_with_planner", "r2c_fft_f32_any_with_planner",
     "c2r_fft_f64_any_with_planner", "c2r_fft_f32_any_with_planner", "r2c_any_batch", "c2r_any_batch",
+    "fft_64_interleaved_any_with_planner", "fft_32_interleaved_any_with_planner", "fft_interleaved_any_batch",
 ]
 
 
@@ -775,6 +776,60 @@ def fft_any_batch(reals, imags, direction: Direction, planner, batch: int, batch
     _check_batch_len("tensors", nr, batch, stride, n)
     check(fn("phastft_fft_any_{s}_dev", planner._sfx)(planner._h, pr, pi, int(direction), int(batch), stride,
                                                       _torch_stream(reals)))
+
+
+def _complex_any_ptr(sfx, signal, planner, host):
+    """The pointer and length of an interleaved complex signal for planner (a PlannerAny of precision sfx): a torch CUDA
+    complex tensor, or with host=True also a numpy array.  Raises before anything reaches the library."""
+    if planner._sfx != sfx:
+        raise TypeError("planner precision does not match the function")
+    if _is_torch(signal):
+        import torch
+        if not signal.is_cuda or signal.dtype != (torch.complex128 if sfx == "f64" else torch.complex64):
+            raise TypeError("expected a CUDA complex tensor of the planner's precision")
+        if signal.dim() != 1 or not signal.is_contiguous():
+            raise TypeError("expected a contiguous 1-D tensor")
+        # (torch keeps a complex tensor's storage offset in whole elements, so its pointer is pair-aligned)
+        return C.c_void_p(signal.data_ptr()), signal.numel()
+    if not host:
+        raise TypeError("expected a torch CUDA complex tensor")
+    cdtype = np.complex128 if sfx == "f64" else np.complex64
+    if not isinstance(signal, np.ndarray) or signal.dtype != cdtype or signal.ndim != 1 or not signal.flags.c_contiguous:
+        raise TypeError(f"expected a contiguous 1-D {np.dtype(cdtype)} array or a torch CUDA complex tensor")
+    if not signal.flags.writeable:
+        raise ValueError("signal is read-only")
+    return signal.ctypes.data_as(C.c_void_p), signal.size
+
+
+def _fft_interleaved_any_with_planner(sfx, signal, direction, planner):
+    p, n = _complex_any_ptr(sfx, signal, planner, True)
+    if n != planner.num_points:
+        raise PhastFTPanic(3)
+    if _is_torch(signal):
+        check(fn("phastft_fft_interleaved_any_{s}_dev", sfx)(planner._h, p, int(direction), 1, n, _torch_stream(signal)))
+    else:
+        check(fn("phastft_fft_interleaved_any_{s}_host", sfx)(planner._h, p, n, int(direction)))
+
+
+def fft_64_interleaved_any_with_planner(signal, direction: Direction, planner: PlannerAny64) -> None:
+    """fft_64_any_with_planner on interleaved complex128 values, in place: a numpy array (synchronous) or a torch CUDA tensor
+    (torch's current stream).  Bluestein and mixed-radix plans give the planar call's results bit for bit."""
+    _fft_interleaved_any_with_planner("f64", signal, direction, planner)
+
+
+def fft_32_interleaved_any_with_planner(signal, direction: Direction, planner: PlannerAny32) -> None:
+    _fft_interleaved_any_with_planner("f32", signal, direction, planner)
+
+
+def fft_interleaved_any_batch(signal, direction: Direction, planner, batch: int, batch_stride: int | None = None) -> None:
+    """fft_any_batch on a flat 1-D torch CUDA complex tensor: `batch` signals of planner.num_points, transform b at complex
+    element b * batch_stride (default planner.num_points)."""
+    n = planner.num_points
+    stride = n if batch_stride is None else int(batch_stride)
+    p, total = _complex_any_ptr(planner._sfx, signal, planner, False)
+    _check_batch_len("tensor", total, batch, stride, n)
+    check(fn("phastft_fft_interleaved_any_{s}_dev", planner._sfx)(planner._h, p, int(direction), int(batch), stride,
+                                                                  _torch_stream(signal)))
 
 
 # ----------------------------------------------------------------------------------------------

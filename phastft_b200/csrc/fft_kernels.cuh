@@ -932,9 +932,9 @@ template <> struct Cx16<float> {
 
 template <typename T>
 struct ChirpParams {
-    const T* in_re;                // CHIRP-PRE: the caller's planar input (re / im swapped for the reverse direction)
-    const T* in_im;
-    T* out_re;                     // CHIRP-POST: the caller's planar output (swapped like the input)
+    const T* in_re;                // CHIRP-PRE: the caller's planar input (re / im swapped for the reverse direction); the
+    const T* in_im;                // interleaved modes read Complex<T> values from in_re (in_im unused)
+    T* out_re;                     // CHIRP-POST: the caller's planar output (swapped like the input), or interleaved as in_re
     T* out_im;
     cx<T>* ws;                     // members x M interleaved complex
     const cx<T>* chirp;            // w[0 .. N), padded with zeros to a multiple of Cx16<T>::V
@@ -954,7 +954,25 @@ struct ChirpParams {
 //   R2C_DIRECT   odd N = L: real x in; bins 0 .. floor(N/2) out
 //   C2R_HALVED   bins 0 .. L in, the c2r pre-processing with W_N^m (swapped); the pairs (y[2k], y[2k+1]) out
 //   C2R_DIRECT   bins 0 .. floor(N/2) in, the Hermitian extension (swapped); the real part of the inverse out
-enum ChirpMode { CHIRP_C2C, CHIRP_R2C_HALVED, CHIRP_R2C_DIRECT, CHIRP_C2R_HALVED, CHIRP_C2R_DIRECT };
+//   C2C_IL       interleaved complex in and out (phastft_fft_interleaved_any_*), the forward direction
+//   C2C_IL_SWAP  the same for the reverse direction: re / im swapped on load and on store, as the planar call swaps its pointers
+enum ChirpMode { CHIRP_C2C, CHIRP_R2C_HALVED, CHIRP_R2C_DIRECT, CHIRP_C2R_HALVED, CHIRP_C2R_DIRECT, CHIRP_C2C_IL, CHIRP_C2C_IL_SWAP };
+
+// The interleaved modes' ends.  The swap is part of the mode, so no kernel carries a runtime test for it.  The caller's array is
+// accessed one complex value at a time: a member starts at any complex offset, so f32 members are only 8-byte aligned.
+template <int MODE>
+__host__ __device__ constexpr bool chirp_il() { return MODE == CHIRP_C2C_IL || MODE == CHIRP_C2C_IL_SWAP; }
+template <typename T, int MODE>
+__device__ __forceinline__ cx<T> il_load(const cx<T>& v) {
+    if constexpr (MODE == CHIRP_C2C_IL_SWAP) return make_cx<T>(v.y, v.x);
+    else return v;
+}
+// the planar call's two stores re = v.x * scale, im = v.y * scale (swapped pointers for the reverse direction) as one
+template <typename T, int MODE>
+__device__ __forceinline__ cx<T> il_store(const cx<T>& v, T scale) {
+    if constexpr (MODE == CHIRP_C2C_IL_SWAP) return make_cx<T>(v.y * scale, v.x * scale);
+    else return make_cx<T>(v.x * scale, v.y * scale);
+}
 
 // CHIRP-POST's items per member: values, or bin pairs (k, L - k) for R2C_HALVED
 template <int MODE>
@@ -1046,6 +1064,11 @@ __global__ void __launch_bounds__(256) chirp_pre_kernel(const __grid_constant__ 
                 const T x = m0 + j < p.n ? re[m0 + j] : T(0);
                 a[j] = make_cx<T>(x * w[j].x, x * w[j].y);
             }
+        } else if constexpr (chirp_il<MODE>()) {
+            const cx<T>* x = reinterpret_cast<const cx<T>*>(p.in_re + (long long)mb * p.bstride);
+#pragma unroll
+            for (int j = 0; j < P::V; ++j)
+                a[j] = m0 + j < p.n ? cmul<T>(il_load<T, MODE>(x[m0 + j]), w[j]) : make_cx<T>(T(0), T(0));
         } else {
 #pragma unroll
             for (int j = 0; j < P::V; ++j)
@@ -1096,6 +1119,13 @@ __global__ void __launch_bounds__(256) chirp_post_kernel(const __grid_constant__
             const cx<T> x = cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y));
             re[k0 + j] = x.x * p.scale;
             im[k0 + j] = x.y * p.scale;
+        }
+    } else if constexpr (chirp_il<MODE>()) {
+        cx<T>* y = reinterpret_cast<cx<T>*>(p.out_re + (long long)mb * p.out_bstride);
+#pragma unroll
+        for (int j = 0; j < P::V; ++j) {
+            if (k0 + j >= p.n) break;
+            y[k0 + j] = il_store<T, MODE>(cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y)), p.scale);
         }
     } else if constexpr (MODE == CHIRP_R2C_HALVED) {
         // bin pair (k, L - k): Z[k] = w[k] conj C[k] and Z[L - k] (Z[L] = Z[0]), then r2c_untangle_kernel's formula with W_N^k;
@@ -1166,7 +1196,8 @@ __global__ void __launch_bounds__(256) chirp_narrow_kernel(const double2* __rest
 // The real any-length plan runs the same kernels with a ChirpMode at both ends (N below is the mixed length: L = N_real / 2
 // for the halved modes, N_real for the direct ones): SMOOTH-PRE loads what CHIRP-PRE would (the pairs, the real data, the c2r
 // pre-processing with W_(2L)^m, the Hermitian extension), the last ODD pass stores the pairs, the real part or the bins up to
-// floor(N/2), and the halved r2c untangles the bins in place afterwards (SMOOTH-POST-R2C).  Pass A is always C2C.
+// floor(N/2), and the halved r2c untangles the bins in place afterwards (SMOOTH-POST-R2C).  The interleaved complex modes
+// (C2C_IL, C2C_IL_SWAP) load and store Complex<T> values of the caller's array instead of planar ones.  Pass A is always C2C.
 // ---------------------------------------------------------------------------------------------
 enum OddRole { ODD_SINGLE, ODD_A, ODD_B };
 constexpr int ODD_MAX_STAGES = 6;      // 3^6 = 729
@@ -1177,15 +1208,15 @@ template <typename T>
 struct OddParams {
     const cx<T>* ws;               // batch x N interleaved: every pass reads it, pass A writes it
     cx<T>* ws_out;
-    T* out_re;                     // the last pass: the caller's planar arrays (re / im swapped for the reverse direction)
-    T* out_im;
+    T* out_re;                     // the last pass: the caller's planar arrays (re / im swapped for the reverse direction), or
+    T* out_im;                     // its interleaved array in out_re
     const cx<T>* wn_hi;            // W_N^(j << lo_bits)
     const cx<T>* wn_lo;            // W_N^j, j < 2^lo_bits
     const cx<T>* wr;               // W_R^j, j < R: the twiddles between the stages of this pass
     const unsigned short* perm;    // tile kernel: where stage 1 puts the butterfly of row r < R / rad[0] (digit reversal)
     long long n, p, cols, total;   // N, P, columns per member (N / R), batch * cols
     long long in_rs, out_rs;       // elements between rows
-    long long bstride;             // elements between members of the caller's arrays
+    long long bstride;             // elements between members of the caller's arrays (complex values for C2R_HALVED and C2C_IL*)
     int role, r, qb, lo_bits;
     int nstages, rad[ODD_MAX_STAGES];
     int cw;                        // tile kernel: columns per CTA
@@ -1200,7 +1231,8 @@ struct OddCol {
     cx<T>* out_c;
     T* out_re;
     T* out_im;
-    cx<T>* out_y;                      // C2R_HALVED: the caller's real array as pairs (bstride counts pairs)
+    cx<T>* out_y;                      // C2R_HALVED: the caller's real array as pairs (bstride counts pairs); C2C_IL*: its
+                                       // interleaved array
     int kmax;                          // R2C_DIRECT: the last row whose output index c + k out_rs is a stored bin (<= N/2)
     unsigned long long e0, de;
     __device__ __forceinline__ OddCol(const OddParams<T>& p, long long g) {
@@ -1212,7 +1244,7 @@ struct OddCol {
         out_c = p.ws_out + m * p.n + c;
         out_re = p.out_re + m * p.bstride + c;
         out_im = p.out_im + m * p.bstride + c;
-        if constexpr (MODE == CHIRP_C2R_HALVED) out_y = reinterpret_cast<cx<T>*>(p.out_re) + m * p.bstride + c;
+        if constexpr (MODE == CHIRP_C2R_HALVED || chirp_il<MODE>()) out_y = reinterpret_cast<cx<T>*>(p.out_re) + m * p.bstride + c;
         if constexpr (MODE == CHIRP_R2C_DIRECT) kmax = (int)((p.n / 2 - c) / p.out_rs);      // c < N / 3 on the last pass
     }
     // row r, times W_N^(e0 + r de)
@@ -1230,6 +1262,8 @@ struct OddCol {
             out_y[k * p.out_rs] = make_cx<T>(v.y * p.scale, v.x * p.scale);      // (y[2K], y[2K+1]) = swap(v) / L
         } else if constexpr (MODE == CHIRP_C2R_DIRECT) {
             out_re[k * p.out_rs] = v.y * p.scale;                               // the real part of the inverse, / N
+        } else if constexpr (chirp_il<MODE>()) {
+            out_y[k * p.out_rs] = il_store<T, MODE>(v, p.scale);
         } else {
             // R2C_DIRECT: the caller holds bins 0 .. floor(N/2) only
             if (MODE == CHIRP_R2C_DIRECT && k > kmax) return;
@@ -1364,12 +1398,12 @@ bool launch_odd_kernel(const OddParams<T>& q, int r, size_t smem, unsigned grid,
 
 // SMOOTH-PRE: ws[m N + n_o P + n_2] = (re, im)[m bstride + n_o + Q n_2].  A block transposes a tile of tq values of n_o by
 // tp values of n_2 through shared memory: it reads runs of tq adjacent elements and writes runs of tp adjacent complex values
-// (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).  The real modes load element n of z instead
-// (bstride is the input's member stride in T either way).
+// (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).  The real modes load element n of z instead, the
+// interleaved ones complex value n of in_re (bstride is the input's member stride in T either way).
 constexpr int SMOOTH_TILE = 1024;
 template <typename T>
 struct SmoothParams {
-    const T* in_re;                // swapped for the reverse direction
+    const T* in_re;                // swapped for the reverse direction; C2C_IL*: the caller's interleaved array (in_im unused)
     const T* in_im;
     cx<T>* ws;
     long long n, p, q, bstride;
@@ -1408,6 +1442,7 @@ __global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__
         if (o + jo < p.q) {
             const long long src = o + jo + p.q * (a + j2);
             if constexpr (MODE == CHIRP_C2C) sm[jo * pitch + j2] = make_cx<T>(re[src], im[src]);
+            else if constexpr (chirp_il<MODE>()) sm[jo * pitch + j2] = il_load<T, MODE>(reinterpret_cast<const cx<T>*>(re)[src]);
             else sm[jo * pitch + j2] = smooth_real_in<T, MODE>(p, re, im, src);
         }
     }

@@ -2512,11 +2512,12 @@ int32_t build_mixed(Mixed<T>& mx, size_t n, const MixedSplit& split, int device)
     CUDA_TRY(cudaFuncSetAttribute(odd_tile_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                   ODD_MAX_ROWS * 128));
     CUDA_TRY(mixed_real_init<T>());
+    CUDA_TRY(any_il_init<T>());
     return mx.w.init(n);                               // room for one member; batched calls grow it
 }
 
 // One ODD pass over `batch` members, MODE the last pass's store (C2C for pass A).  Launch record: R = rows, C = the columns a
-// CTA covers; the kind carries -C2R / -R2C for the real stores.
+// CTA covers; the kind carries -C2R / -R2C for the real stores, -IL for the interleaved ones.
 template <int MODE, typename T>
 int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cudaStream_t stream) {
     const OddPass<T>& ps = mx.pass[i];
@@ -2536,10 +2537,13 @@ int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cuda
     if (blocks > 0x7fffffffu) return fail(PHASTFT_ERR_INVALID_ARG, "batch * N is too large for one launch of the odd pass");
     const size_t smem = ps.cw ? (size_t)ps.r * ps.cw * sizeof(cx<T>) : 0;
     const bool ok = MODE == CHIRP_C2C ? launch_odd_kernel<T, CHIRP_C2C>(q, ps.r, smem, (unsigned)blocks, stream)
-                                      : launch_odd_real<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream);
+                    : chirp_il<MODE>() ? launch_odd_il<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream)
+                                       : launch_odd_real<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream);
     if (!ok) return fail(PHASTFT_ERR_INVALID_ARG, "no register kernel of " + std::to_string(ps.r) + " rows");
     CUDA_TRY(cudaGetLastError());
-    const char* name = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT ? "ODD-C2R" : MODE == CHIRP_R2C_DIRECT ? "ODD-R2C" : "ODD";
+    const char* name = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT ? "ODD-C2R" : MODE == CHIRP_R2C_DIRECT ? "ODD-R2C"
+                       : chirp_il<MODE>()                                   ? "ODD-IL"
+                                                                            : "ODD";
     note_launch({name, ps.r, 0, cover, ODD_NT, 0, ps.cw ? "tile" : "reg", false});
     return PHASTFT_OK;
 }
@@ -2573,14 +2577,16 @@ int32_t build_two_level(TwoLevelRoots<T>& t, size_t n, size_t count) {
 }
 
 // One mixed-radix call of `batch` members: SMOOTH-PRE, the P-point plan on Q * batch workspace members, the ODD pass(es), with
-// the ends in MODE (CHIRP_C2C for the complex plan; the real modes as in CHIRP-PRE / CHIRP-POST, fft_kernels.cuh).  in / out
-// are the caller's arrays, swapped for the reverse direction; in_bstride counts T, out_bstride what the last pass stores (T,
-// or pairs for C2R_HALVED); scale is 1, 1/N or 1/L.  `wn` is the real plan's W_(2L) for the halved modes.  The halved r2c ends
-// with SMOOTH-POST-R2C on the bins.  The workspace follows AnyWorkspace's protocol (`reserve_fn` names the call that grows it).
+// the ends in MODE (CHIRP_C2C for the complex plan, C2C_IL / C2C_IL_SWAP for its interleaved calls; the real modes as in
+// CHIRP-PRE / CHIRP-POST, fft_kernels.cuh).  in / out are the caller's arrays, swapped for the reverse direction (the
+// interleaved modes: in_re and out_re, swapped by the mode); in_bstride counts T, out_bstride what the last pass stores (T, or
+// complex values for C2R_HALVED and the interleaved modes); scale is 1, 1/N or 1/L.  `wn` is the real plan's W_(2L) for the
+// halved modes.  The halved r2c ends with SMOOTH-POST-R2C on the bins.  The workspace follows AnyWorkspace's protocol (`reserve_fn` names the call that grows it).
 template <int MODE, typename T>
 int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_bstride, T* out_re, T* out_im, size_t out_bstride,
                   T scale, size_t batch, cudaStream_t stream, const char* reserve_fn, const TwoLevelRoots<T>* wn = nullptr) {
     constexpr bool r2c = MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT, c2r = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT;
+    constexpr bool il = chirp_il<MODE>();
     constexpr int LAST = MODE == CHIRP_R2C_HALVED ? CHIRP_C2C : MODE;   // the halved r2c stores Z, then untangles it in place
     DeviceGuard g(mx.device);
     const size_t P = mx.split.p, Q = (size_t)mx.split.qa * mx.split.qb;
@@ -2607,9 +2613,11 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
         s2.in_re += done * in_bstride; s2.ws += done * mx.n;
         if (s2.in_im) s2.in_im += done * in_bstride;
         if constexpr (MODE == CHIRP_C2C) smooth_pre_kernel<T><<<(unsigned)(nb * sp.tiles_per_member), 256, 0, stream>>>(s2);
+        else if constexpr (il) launch_smooth_pre_il<T>(MODE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
         else launch_smooth_pre_real<T>(MODE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
         CUDA_TRY(cudaGetLastError());
-        note_launch({r2c ? "SMOOTH-PRE-R2C" : c2r ? "SMOOTH-PRE-C2R" : "SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0, "plain", false});
+        note_launch({r2c ? "SMOOTH-PRE-R2C" : c2r ? "SMOOTH-PRE-C2R" : il ? "SMOOTH-PRE-IL" : "SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0,
+                     "plain", false});
     }
     if (P > 1) {
         Io<T> io;
@@ -2669,10 +2677,11 @@ struct PlanAny {
     mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then the workspace's mu)
     mutable T* stage_re = nullptr;     // host-API staging: N each
     mutable T* stage_im = nullptr;
+    mutable T* stage_il = nullptr;     // the interleaved host calls' staging: N complex, allocated by the first such call
     std::string description;
     ~PlanAny() {
         DeviceGuard g(device);
-        for (void* p : {(void*)stage_re, (void*)stage_im})
+        for (void* p : {(void*)stage_re, (void*)stage_im, (void*)stage_il})
             if (p) cudaFree(p);
         delete pow2;
     }
@@ -2810,12 +2819,13 @@ enum ChirpKind { CHIRP_PRE, CHIRP_MUL, CHIRP_POST };
 
 // One CHIRP-* kernel over `members` batch members, `per` threads each: a member-major grid of 256-thread blocks (as launch_real),
 // several launches when it would exceed 2^31 - 1 blocks.  Launch record: R = M, C = the members of that launch; the kind carries
-// -R2C / -C2R for the real modes' CHIRP-PRE and CHIRP-POST.
+// -R2C / -C2R for the real modes' CHIRP-PRE and CHIRP-POST, -IL for the interleaved ones.
 template <int MODE, typename T>
 int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_t members, cudaStream_t stream) {
     const size_t bpm = (per + 255) / 256;
     const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
     constexpr bool r2c = MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT, c2r = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT;
+    constexpr bool il = chirp_il<MODE>();
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
         ChirpParams<T> q = cp;
@@ -2831,13 +2841,14 @@ int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_
         q.ws += done << cp.log2m;
         q.blocks_per_member = (unsigned)bpm;
         const dim3 grid((unsigned)(nb * bpm));
-        if (kind == CHIRP_PRE) chirp_pre_kernel<T, MODE><<<grid, 256, 0, stream>>>(q);
-        else if (kind == CHIRP_MUL) chirp_mul_kernel<T><<<grid, 256, 0, stream>>>(q);
+        if (kind == CHIRP_MUL) chirp_mul_kernel<T><<<grid, 256, 0, stream>>>(q);
+        else if constexpr (il) launch_chirp_il<T>(MODE, kind == CHIRP_POST, q, grid.x, stream);
+        else if (kind == CHIRP_PRE) chirp_pre_kernel<T, MODE><<<grid, 256, 0, stream>>>(q);
         else chirp_post_kernel<T, MODE><<<grid, 256, 0, stream>>>(q);
         CUDA_TRY(cudaGetLastError());
         const char* name = kind == CHIRP_MUL ? "CHIRP-MUL"
-                           : kind == CHIRP_PRE ? (r2c ? "CHIRP-PRE-R2C" : c2r ? "CHIRP-PRE-C2R" : "CHIRP-PRE")
-                                               : (r2c ? "CHIRP-POST-R2C" : c2r ? "CHIRP-POST-C2R" : "CHIRP-POST");
+                           : kind == CHIRP_PRE ? (r2c ? "CHIRP-PRE-R2C" : c2r ? "CHIRP-PRE-C2R" : il ? "CHIRP-PRE-IL" : "CHIRP-PRE")
+                                               : (r2c ? "CHIRP-POST-R2C" : c2r ? "CHIRP-POST-C2R" : il ? "CHIRP-POST-IL" : "CHIRP-POST");
         note_launch({name, 1 << cp.log2m, 0, (int)nb, 256, 0, "plain", false});
     }
     return PHASTFT_OK;
@@ -2901,6 +2912,31 @@ int32_t any_dev(const PlanAny<T>* pl, T* d_re, T* d_im, int direction, size_t ba
     return bluestein_run<CHIRP_C2C>(pl->bs, cp, batch, stream, "phastft_plan_any_*_reserve");
 }
 
+// interleaved, in place, device pointers: the semantics of any_dev on Complex<T> members b * bstride complex values apart.  The
+// Bluestein and mixed paths run any_dev's kernels with the interleaved modes at the ends (bit-identical results); powers of
+// two run fft_interleaved_dev.
+template <typename T>
+int32_t any_interleaved_dev(const PlanAny<T>* pl, T* d_sig, int direction, size_t batch, size_t bstride, cudaStream_t stream) {
+    if (!pl || !d_sig) return fail(PHASTFT_ERR_INVALID_ARG, "NULL argument");
+    if (direction != PHASTFT_FORWARD && direction != PHASTFT_REVERSE) return fail(PHASTFT_ERR_INVALID_ARG, "direction must be 1 or -1");
+    if (batch > 1 && bstride < pl->n) return fail(PHASTFT_ERR_INVALID_ARG, "batch_stride < N");
+    if (int32_t st = check_pair_alignment(d_sig, "d_signal")) return st;
+    if (pl->pow2) return fft_interleaved_dev(pl->pow2, d_sig, direction, batch, bstride, stream);
+    if (batch == 0) return PHASTFT_OK;
+    const bool fwd = direction == PHASTFT_FORWARD;
+    const T scale = fwd ? T(1) : T(1) / (T)pl->n;
+    const char* res = "phastft_plan_any_*_reserve";
+    if (pl->mx.inner)
+        return fwd ? mixed_run<CHIRP_C2C_IL, T>(pl->mx, d_sig, nullptr, 2 * bstride, d_sig, nullptr, bstride, scale, batch, stream, res)
+                   : mixed_run<CHIRP_C2C_IL_SWAP, T>(pl->mx, d_sig, nullptr, 2 * bstride, d_sig, nullptr, bstride, scale, batch, stream, res);
+    ChirpParams<T> cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.in_re = cp.out_re = d_sig;
+    cp.bstride = cp.out_bstride = 2 * (long long)bstride;
+    cp.scale = scale;
+    return fwd ? bluestein_run<CHIRP_C2C_IL>(pl->bs, cp, batch, stream, res) : bluestein_run<CHIRP_C2C_IL_SWAP>(pl->bs, cp, batch, stream, res);
+}
+
 template <typename T>
 int32_t any_reserve(const PlanAny<T>* pl, size_t batch) {
     if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
@@ -2932,6 +2968,30 @@ int32_t any_host(const PlanAny<T>* pl, T* re, size_t len_re, T* im, size_t len_i
     if (int32_t st = any_dev(pl, pl->stage_re, pl->stage_im, direction, 1, pl->n, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(re, pl->stage_re, bytes, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(im, pl->stage_im, bytes, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
+// an interleaved host slice of N complex values: H2D, run, D2H, synchronous
+template <typename T>
+int32_t any_interleaved_host(const PlanAny<T>* pl, T* sig, size_t len_complex, int direction) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (len_complex != pl->n)
+        return fail(PHASTFT_ERR_PLAN_MISMATCH, "slice length " + std::to_string(len_complex) + ", plan n = " + std::to_string(pl->n));
+    if (direction != PHASTFT_FORWARD && direction != PHASTFT_REVERSE) return fail(PHASTFT_ERR_INVALID_ARG, "direction must be 1 or -1");
+    if (!sig) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    if (pl->pow2) return fft_interleaved_host(pl->pow2, sig, len_complex, direction);
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    {
+        std::lock_guard<std::mutex> lock(pl->workspace().mu);   // released before any_interleaved_dev, which takes it
+        if (!pl->stage_il) CUDA_TRY(cudaMalloc(&pl->stage_il, 2 * pl->n * sizeof(T)));
+    }
+    cudaStream_t s = pl->host_stream();
+    const size_t bytes = 2 * pl->n * sizeof(T);
+    CUDA_TRY(cudaMemcpyAsync(pl->stage_il, sig, bytes, cudaMemcpyHostToDevice, s));
+    if (int32_t st = any_interleaved_dev(pl, pl->stage_il, direction, 1, pl->n, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(sig, pl->stage_il, bytes, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return PHASTFT_OK;
 }
@@ -3436,6 +3496,15 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                          int dir) {                                                                     \
         launches_reset();                                                                                               \
         return any_host<T>(AS_CANY(T, p), re, lre, im, lim, dir);                                                       \
+    }                                                                                                                   \
+    int32_t phastft_fft_interleaved_any_##SFX##_dev(const phastft_plan_any_##SFX* p, T* sig, int dir, size_t batch,    \
+                                                    size_t bstride, void* s) {                                          \
+        launches_reset();                                                                                               \
+        return any_interleaved_dev<T>(AS_CANY(T, p), sig, dir, batch, bstride, (cudaStream_t)s);                        \
+    }                                                                                                                   \
+    int32_t phastft_fft_interleaved_any_##SFX##_host(const phastft_plan_any_##SFX* p, T* sig, size_t len, int dir) {    \
+        launches_reset();                                                                                               \
+        return any_interleaved_host<T>(AS_CANY(T, p), sig, len, dir);                                                   \
     }                                                                                                                   \
     int32_t phastft_plan_r2c_any_##SFX##_create(size_t n, int device, phastft_plan_r2c_any_##SFX** out) {               \
         PlanR2cAny<T>* pl = nullptr;                                                                                    \

@@ -3,7 +3,7 @@
 // The kernels are instantiated in several translation units so the library builds in parallel
 // (__graft_entry__.build()): reg_strided.cu (COL / TRANS passes, compiled once per precision and kind),
 // reg_row.cu (whole-transform-in-one-CTA kernels), reg_multi.cu (cluster and pipelined two-pass launches), mixed_real.cu (the
-// real modes of the mixed-radix kernels).
+// real modes of the mixed-radix kernels), any_interleaved.cu (the interleaved complex modes of the any-length end kernels).
 // phastft_cuda.cu holds the planner, the launcher and the C ABI and only sees these descriptors.
 #pragma once
 #include <string>
@@ -127,5 +127,12 @@ template <typename T> cudaError_t mixed_real_init();
 template <typename T> bool launch_odd_real(int mode, const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
 template <typename T> void launch_smooth_pre_real(int mode, const SmoothParams<T>& p, unsigned grid, cudaStream_t stream);
 template <typename T> void launch_smooth_post_r2c(const SmoothPostParams<T>& p, unsigned grid, cudaStream_t stream);
+
+// defined in any_interleaved.cu: the same for the interleaved complex modes (`mode` CHIRP_C2C_IL or CHIRP_C2C_IL_SWAP) of
+// SMOOTH-PRE, the last ODD pass and CHIRP-PRE / CHIRP-POST (`post`)
+template <typename T> cudaError_t any_il_init();
+template <typename T> bool launch_odd_il(int mode, const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_smooth_pre_il(int mode, const SmoothParams<T>& p, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_chirp_il(int mode, bool post, const ChirpParams<T>& p, unsigned grid, cudaStream_t stream);
 
 }  // namespace phast

@@ -404,6 +404,32 @@ mod interleaved {
         let planner = PlannerDit32::new(signal.len());
         fft_32_interleaved_with_planner(signal, direction, &planner);
     }
+
+    // Additive: interleaved transforms of any length on the any-length planners
+    macro_rules! impl_interleaved_any {
+        ($with_planner:ident, $device_batch:ident, $t:ty, $planner:ident, $ffi_host:ident, $ffi_dev:ident) => {
+            /// In place on `planner.num_points()` interleaved host values, any length; forward unscaled, reverse scaled by 1/N.
+            /// Bluestein and mixed-radix plans give the planar call's results bit for bit.  Panics on a length mismatch.
+            pub fn $with_planner(signal: &mut [Complex<$t>], direction: Direction, planner: &$planner) {
+                check(unsafe { ffi::$ffi_host(planner.raw, signal.as_mut_ptr() as *mut $t, signal.len(), direction as i32) });
+            }
+            /// Device-resident interleaved data, `batch` transforms at complex element `b * batch_stride` (batch_stride >= N),
+            /// stream-ordered on `stream`; allocates only when the plan's workspace must grow (see `reserve`).
+            ///
+            /// # Safety
+            /// `d_signal` must be a device pointer, aligned to `Complex<T>`, valid for `(batch - 1) * batch_stride + n` complex
+            /// values on the planner's device, and must not be used by other work on other streams until this call's work has
+            /// completed.
+            pub unsafe fn $device_batch(d_signal: *mut Complex<$t>, direction: Direction, planner: &$planner, batch: usize,
+                                        batch_stride: usize, stream: *mut std::os::raw::c_void) {
+                check(ffi::$ffi_dev(planner.raw, d_signal as *mut $t, direction as i32, batch, batch_stride, stream));
+            }
+        };
+    }
+    impl_interleaved_any!(fft_64_interleaved_any_with_planner, fft_64_interleaved_any_device_batch, f64, PlannerAny64,
+                          phastft_fft_interleaved_any_f64_host, phastft_fft_interleaved_any_f64_dev);
+    impl_interleaved_any!(fft_32_interleaved_any_with_planner, fft_32_interleaved_any_device_batch, f32, PlannerAny32,
+                          phastft_fft_interleaved_any_f32_host, phastft_fft_interleaved_any_f32_dev);
 }
 #[cfg(feature = "complex-nums")]
 pub use interleaved::*;
