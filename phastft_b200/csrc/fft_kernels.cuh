@@ -60,7 +60,9 @@ struct PassParams {
     Tw2 tw2;                       // two-level W_N table
     const cx<T>* __restrict__ tw_stage;  // W_R^e, e < R           (stage twiddles)
     const cx<T>* __restrict__ tw_stage_im;  // KIND_ROW: per stage s >= 1 the table [i][m] = W_L^(m*i), L = Ns(s)*rad(s), concatenated
-                                         // (lanes run along m in a one-CTA kernel: consecutive lanes read consecutive entries)
+                                         // (lanes run along m in a one-CTA kernel: consecutive lanes read consecutive entries);
+                                         // KIND_COL / KIND_TRANS with a radix-32 last stage: its table [m][i] = W_R^(m*i), i < 32
+                                         // (stage32_table_kernel); otherwise unused
     const cx<T>* __restrict__ tw_wc;     // KIND_TRANS, 2-pass plans: W_L^(c*m), [c][m] layout
     T scale;                       // multiplied into the stored result (1/N for the inverse)
     // cluster exchange (XCH = 1 producer only): the consuming pass's tile is [CB rows][P2 points]
@@ -197,6 +199,9 @@ struct PassKernel {
     static constexpr int TILE_ELEMS = (S >= 2) ? R * C : 0;
     static constexpr int G_ELEMS = (KIND == KIND_TRANS) ? C * R1 : R1;
     static constexpr bool ASYNC_IN = (XCH == MODE_TMA_IN || XCH == MODE_BULK_IN || XCH == MODE_ROW_BULK);
+    // strided tiles whose last stage is radix 32 (1024 = 32 x 32, 512 = 16 x 32): that stage reads W_R^(m*i) from the plan's
+    // [m][i] table (PassParams::tw_stage_im), and stage 1 is written as a single trip when it can be (see body())
+    static constexpr bool STAGE32 = KIND != KIND_ROW && S >= 2 && RL::rad(S - 1) == 32;
     static constexpr size_t TABLE_END = sizeof(cx<T>) * (size_t)(TILE_ELEMS + M + G_ELEMS);
     static constexpr size_t MBAR_OFF = (TABLE_END + 15) & ~size_t(15);
     static constexpr size_t OUT_OFF = (MBAR_OFF + 16 + 127) & ~size_t(127);      // MODE_ROW_BULK: planar output staging [2][C][R]
@@ -371,6 +376,14 @@ struct PassKernel {
                     else w[i] = ctwid<T>(w[hi], w[i - hi]);
                     x[i] = ctwid<T>(x[i], w[i]);
                 }
+            } else if constexpr (STAGE32 && LAST) {
+                // The product chain below would keep up to 15 complex twiddles live beside the 32 values and spill the
+                // 1024-row tiles on sm_90a.  Its results for every m come instead from the plan's [m][i] table, which
+                // stage32_table_kernel fills with that same chain (bit-identical values): 31 loads (L1-resident), no products.
+                static_assert(RAD == 32 && NS * RAD == R, "the radix-32 table holds the tile's last stage");
+                const cx<T>* tws = p.tw_stage_im + m * RAD;
+#pragma unroll
+                for (int i = 1; i < RAD; ++i) x[i] = ctwid<T>(x[i], __ldg(tws + i));
             } else {
 #if PHAST_EXP_STAGE_TW == 1      // experiment: no stage twiddles (wrong results; prices them)
 #elif PHAST_EXP_STAGE_TW == 2    // experiment: the round-1 form, one table load per twiddle
@@ -694,6 +707,9 @@ struct PassKernel {
                         else gstore_n<R1>(p, out_base + c, out_kstride, x);
                     }
                 }
+                // A preloaded task is the thread's only one, but the compiler cannot prove the loop runs once: pre[] then has to
+                // outlive x[] across the back edge, and in the 32 x 32 tiles the two 32-value arrays do not fit the registers.
+                if constexpr (PRELOAD && STAGE32) break;
             }
         };
         if constexpr (PRELOAD || XCH == MODE_C2R_IN) stage1(std::integral_constant<int, 0>{});
@@ -728,6 +744,25 @@ __global__ void __launch_bounds__(NT, MINB) fft_pass_kernel(const __grid_constan
 template <typename T, class RL, int C, int NT, int KIND, int MODE, int VARIANT = 0, int MINB = 0>
 __global__ void __launch_bounds__(NT, MINB) fft_pass_async_kernel(const __grid_constant__ PassParams<T> p) {
     PassKernel<T, RL, C, NT, KIND, MODE, VARIANT>::body(p, blockIdx.x);
+}
+
+// The table a strided tile's radix-32 last stage reads (stage_from_tile): out[m * 32 + i] = W_R^(m*i), m < R / 32, i < 32, out of
+// the pass's W_R table by the product chain that stage computed in registers -- W^(m*i) loaded for i = 1, 2, 4, 8, 16, every other
+// i the product of two earlier ones (i = hi + lo, hi its top bit) -- so each entry is bit for bit what the stage used to multiply by.
+template <typename T>
+__global__ void __launch_bounds__(256) stage32_table_kernel(const cx<T>* __restrict__ tw_stage, cx<T>* __restrict__ out, int ns) {
+    const int m = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+    if (m >= ns) return;
+    cx<T> w[32];
+    w[0] = __ldg(tw_stage);
+#pragma unroll
+    for (int i = 1; i < 32; ++i) {
+        const int hi = 1 << (31 - __builtin_clz((unsigned)i));
+        if (i == hi) w[i] = __ldg(tw_stage + m * i);
+        else w[i] = ctwid<T>(w[hi], w[i - hi]);
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) out[m * 32 + i] = w[i];
 }
 
 // ---------------------------------------------------------------------------------------------

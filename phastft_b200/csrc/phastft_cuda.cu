@@ -222,14 +222,16 @@ constexpr int MAX_PASSES = 3;
 // between ranks (PlannerMode::Tune, PHASTFT_* overrides): import / broadcast compare headers first.
 constexpr size_t BLOB_HEADER_BYTES = 256;
 struct BlobHeader {
-    uint64_t magic;        // "PHASTFT2"
+    uint64_t magic;        // "PASTHFT3" (3: blobs with radix-32 stage tables)
     uint64_t bytes;        // whole blob, header included
     uint64_t n;
     uint32_t precision_bits, num_passes;
     uint64_t layout_sig;   // FNV-1a of the plan description (factors, kernels, radices, variants)
+    uint64_t tw_stage_off[MAX_PASSES];   // per pass: byte offset of its W_R table
+    uint64_t tw32_off[MAX_PASSES];       // ... and of its radix-32 stage table (PassDesc::tw32_off), 0 if it has none
 };
 static_assert(sizeof(BlobHeader) <= BLOB_HEADER_BYTES, "header fits its slot");
-constexpr uint64_t BLOB_MAGIC = 0x3254464854534150ull;
+constexpr uint64_t BLOB_MAGIC = 0x3354464854534150ull;
 inline uint64_t fnv1a(const std::string& str) {
     uint64_t h = 1469598103934665603ull;
     for (unsigned char c : str) { h ^= c; h *= 1099511628211ull; }
@@ -258,6 +260,8 @@ struct PassDesc {
     size_t tw_im_off_b = (size_t)-1;      // ... and for `kb`
     int log2R = 0, log2A = 0, log2B = 0, log2R1 = 0, log2Rprev = 0, has_tw = 0, tw_shift = 0;
     size_t tw_stage_off = 0;  // byte offsets into the table blob
+    size_t tw32_off = (size_t)-1;         // strided passes whose kernels end in a radix-32 stage: that stage's [m][i] = W_R^(m*i)
+                                          // table (R values, filled on the device by stage32_table_kernel from the W_R table)
     size_t tw_wc_off = (size_t)-1;
     size_t tw_wc_off_b = (size_t)-1;      // same table for `kb` (depends on its C and first radix)
 };
@@ -283,7 +287,7 @@ struct Plan {
     int pipe_grid_b = 0, pipe_grid_1 = 0;   // co-resident CTAs of those launches on this device
     mutable unsigned char* pipe_state = nullptr;   // ticket + done1[batch] + done2[batch], zeroed per call
     mutable size_t pipe_state_batch = 0;
-    // table blob: [tw2_hi][tw2_lo][per pass W_R][wc]
+    // table blob: [header][tw2_hi][tw2_lo][per pass W_R, [i][m] / radix-32 stage tables, wc]
     std::vector<unsigned char> blob_host;
     unsigned char* blob_dev = nullptr;
     size_t hi_off = 0, lo_off = 0;
@@ -668,6 +672,16 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
                 if (ends && e.mode == MODE_BULK_IN && e.kind == KIND_TRANS && e.R == (1 << f[2]) && e.C == TileC<T>::CW) pl->pass[2].kt = &e;
             }
     }
+    // The radix-32 stage table of every strided pass that may launch a kernel ending in a radix-32 stage (any of k, kb, kt, kc, kcb)
+    auto ends_in_32 = [](const KernelEntry<T>* k) { return k && k->kind != KIND_ROW && k->stages >= 2 && k->rads[k->stages - 1] == 32; };
+    for (int p = 0; p < pl->num_passes; ++p) {
+        PassDesc<T>& d = pl->pass[p];
+        if (ends_in_32(d.k) || ends_in_32(d.kb) || ends_in_32(d.kt) || ends_in_32(d.kc) || ends_in_32(d.kcb)) {
+            d.tw32_off = off;
+            off += (size_t(1) << d.log2R) * sizeof(cx<T>);
+            off = (off + 255) & ~size_t(255);
+        }
+    }
     // Batches of transforms that one CTA can hold (128 KB tile: 2^13 f64, 2^14 f32) use a one-CTA kernel: one launch,
     // one HBM round trip.  PHASTFT_ONE_CTA_MAX (log2) lowers the limit for re-tuning.
     // 2^13 f64 / 2^13-2^14 f32 in one CTA (64-128 KB tile): slower than two passes of small tiles while the stage twiddles were
@@ -774,6 +788,17 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
     CUDA_TRY(cudaMemcpy(pl->blob_dev, pl->blob_host.data(), pl->blob_host.size(), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaStreamCreateWithFlags(&pl->stream, cudaStreamNonBlocking));
     CUDA_TRY(cudaEventCreateWithFlags(&pl->ws_free, cudaEventDisableTiming));
+    // The radix-32 stage tables, from the W_R tables just copied.  On the default stream: a cudaMemcpy from pageable memory may
+    // return before its data has landed, and only work on that stream is ordered after it.
+    for (int p = 0; p < pl->num_passes; ++p) {
+        const PassDesc<T>& d = pl->pass[p];
+        if (d.tw32_off == (size_t)-1) continue;
+        const int ns = 1 << (d.log2R - 5);
+        stage32_table_kernel<T><<<(ns + 255) / 256, 256>>>(reinterpret_cast<const cx<T>*>(pl->blob_dev + d.tw_stage_off),
+                                                           reinterpret_cast<cx<T>*>(pl->blob_dev + d.tw32_off), ns);
+        CUDA_TRY(cudaGetLastError());
+    }
+    CUDA_TRY(cudaStreamSynchronize(0));
     for (int p = 0; p < pl->num_passes; ++p) {
         CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].k->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].k->smem));
         if (pl->pass[p].kb)
@@ -915,6 +940,10 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
         h.magic = BLOB_MAGIC; h.bytes = pl->blob_host.size(); h.n = n;
         h.precision_bits = 8 * sizeof(T); h.num_passes = (uint32_t)pl->num_passes;
         h.layout_sig = fnv1a(pl->description);
+        for (int p = 0; p < pl->num_passes; ++p) {
+            h.tw_stage_off[p] = pl->pass[p].tw_stage_off;
+            h.tw32_off[p] = pl->pass[p].tw32_off == (size_t)-1 ? 0 : pl->pass[p].tw32_off;
+        }
         memcpy(pl->blob_host.data(), &h, sizeof(h));
         CUDA_TRY(cudaMemcpy(pl->blob_dev, pl->blob_host.data(), BLOB_HEADER_BYTES, cudaMemcpyHostToDevice));
     }
@@ -1037,7 +1066,7 @@ int32_t prepare_pass_desc(const Plan<T>& pl, const PassDesc<T>& d, int p, const 
     prm.tw2.lo_bits = pl.lo_bits;
     prm.tw_stage = reinterpret_cast<const cx<T>*>(pl.blob_dev + d.tw_stage_off);
     const size_t wc_off = use_kt ? d.tw_wc_off_t : many ? d.tw_wc_off_b : d.tw_wc_off;
-    const size_t im_off = many ? d.tw_im_off_b : d.tw_im_off;
+    const size_t im_off = d.tw32_off != (size_t)-1 ? d.tw32_off : many ? d.tw_im_off_b : d.tw_im_off;
     prm.tw_stage_im = im_off == (size_t)-1 ? nullptr : reinterpret_cast<const cx<T>*>(pl.blob_dev + im_off);
     prm.tw_wc = wc_off == (size_t)-1 ? nullptr : reinterpret_cast<const cx<T>*>(pl.blob_dev + wc_off);
     unsigned long long blocks;
@@ -1764,7 +1793,8 @@ int32_t check_blob_header(const Plan<T>* pl, const BlobHeader& h) {
     memcpy(&mine, pl->blob_host.data(), sizeof(mine));
     if (h.magic != BLOB_MAGIC) return fail(PHASTFT_ERR_PLAN_MISMATCH, "table blob: bad magic (not a phastft table blob)");
     if (h.n != mine.n || h.precision_bits != mine.precision_bits) return fail(PHASTFT_ERR_PLAN_MISMATCH, "table blob is for another size / precision");
-    if (h.bytes != mine.bytes || h.num_passes != mine.num_passes || h.layout_sig != mine.layout_sig)
+    if (h.bytes != mine.bytes || h.num_passes != mine.num_passes || h.layout_sig != mine.layout_sig ||
+        memcmp(h.tw_stage_off, mine.tw_stage_off, sizeof(h.tw_stage_off)) || memcmp(h.tw32_off, mine.tw32_off, sizeof(h.tw32_off)))
         return fail(PHASTFT_ERR_PLAN_MISMATCH, "table blob was laid out for a different pass decomposition / kernel choice "
                                                "(PlannerMode::Tune or a PHASTFT_* override on one rank only?)");
     return PHASTFT_OK;

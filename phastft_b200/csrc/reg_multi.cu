@@ -30,6 +30,7 @@ ClusterEntry<T> make_cluster() {
     using PK1 = PassKernel<T, RL1, C1, NT, KIND_COL, 1, 0>;
     using PK2 = PassKernel<T, RL2, C2, NT, KIND_TRANS, 2, 0>;
     static_assert(PK1::TILE_ELEMS == PK2::TILE_ELEMS, "both passes use the same tile");
+    static_assert(!PK1::STAGE32 && !PK2::STAGE32, "the planner builds no radix-32 stage table for cluster launches");
     static_assert(NT % C1 == 0, "a COL thread keeps its column");
     constexpr size_t SMEM = PK1::SMEM_BYTES > PK2::SMEM_BYTES ? PK1::SMEM_BYTES : PK2::SMEM_BYTES;
     static_assert(SMEM <= 227 * 1024, "tile exceeds the 227 KB shared memory of an sm_90 CTA");
