@@ -56,6 +56,12 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
+/* Thread-local, like phastft_last_launches: the bytes of plan-owned scratch (workspaces, c2r scratch, host staging) that the
+ * calling thread's most recent execution call filled with 0xFF bytes (a NaN in f32 and f64) before using them.  Nonzero only
+ * for plans built while the environment variable PHASTFT_SCRIBBLE=1 was set: such plans poison their scratch when it is
+ * allocated and, with cudaMemsetAsync on the call's stream, before each call's first use, so a kernel that reads scratch it has
+ * not written in the same call produces NaN.  A testing aid; it never touches constant tables and changes no result. */
+PHASTFT_API uint64_t phastft_last_scribble_bytes(void);
 /* The *_oneshot entry points (a planner per call, lib.rs:180 / r2c.rs:522,696) keep their most recent plan per
  * precision and reuse it when the next call has the same size and device; this releases those plans and their
  * device buffers. */

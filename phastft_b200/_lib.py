@@ -63,6 +63,7 @@ lib.phastft_last_error.restype = C.c_char_p
 lib.phastft_version.restype = C.c_char_p
 lib.phastft_launch_count.restype = C.c_uint64
 lib.phastft_last_launches.restype = C.c_char_p
+lib.phastft_last_scribble_bytes.restype = C.c_uint64
 lib.phastft_device_count.argtypes = [C.POINTER(_ci)]
 lib.phastft_device_count.restype = _i32
 
@@ -183,6 +184,7 @@ def plan_tune_candidates(n: int, precision_bits: int = 64):
 
 GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization",
                   "phastft_plan_tune_candidates", "phastft_any_mixed_factorization", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
+                  "phastft_last_scribble_bytes",
                   "phastft_device_count", "phastft_options_default", "phastft_options_guess"]
 
 for _name, (_args, _res) in SIGNATURES.items():
@@ -206,6 +208,11 @@ def last_launches() -> list:
     """The kernels this thread's most recent library call launched, one string per launch (include/phastft_cuda.h)."""
     text = (lib.phastft_last_launches() or b"").decode()
     return text.split("; ") if text else []
+
+
+def last_scribble_bytes() -> int:
+    """Bytes of plan scratch this thread's most recent library call poisoned (plans built under PHASTFT_SCRIBBLE=1)."""
+    return int(lib.phastft_last_scribble_bytes())
 
 
 def device_count() -> int:

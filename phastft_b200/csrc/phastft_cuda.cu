@@ -56,7 +56,30 @@ thread_local std::vector<LaunchRec> g_launch_log;
 thread_local std::string g_launch_text;
 thread_local std::string g_r2c_desc_text;   // phastft_plan_r2c_*_describe: built per call (it reads the environment)
 
-void launches_reset() { g_launch_log.clear(); }
+// PHASTFT_SCRIBBLE=1, read when a plan is built: the plan's scratch (workspaces, c2r scratch, host staging) is filled with 0xFF
+// bytes, a NaN in f32 and f64, when it is allocated and, on the call's stream, before each call uses it.  A kernel that reads
+// scratch before writing it in the same call then produces NaN instead of what the previous call left there.  Constant tables
+// are never touched.  phastft_last_scribble_bytes() reports the bytes the calling thread's most recent call poisoned.
+thread_local uint64_t g_scribble_bytes = 0;
+bool scribble_env() {
+    const char* e = getenv("PHASTFT_SCRIBBLE");
+    return e && atoi(e) != 0;
+}
+// before a call's first use of [p, p + bytes), ordered on `stream` (a graph node while the stream is being captured)
+cudaError_t scribble(bool on, void* p, size_t bytes, cudaStream_t stream) {
+    if (!on || !p || !bytes) return cudaSuccess;
+    g_scribble_bytes += bytes;
+    return cudaMemsetAsync(p, 0xFF, bytes, stream);
+}
+// a buffer just allocated: done before any stream can use it
+cudaError_t scribble_new(bool on, void* p, size_t bytes) {
+    if (!on || !p || !bytes) return cudaSuccess;
+    g_scribble_bytes += bytes;
+    cudaError_t e = cudaMemset(p, 0xFF, bytes);
+    return e == cudaSuccess ? cudaDeviceSynchronize() : e;
+}
+
+void launches_reset() { g_launch_log.clear(); g_scribble_bytes = 0; }
 void note_launch(const LaunchRec& r) {
     g_launch_log.push_back(r);
     g_launches.fetch_add(1, std::memory_order_relaxed);
@@ -317,6 +340,7 @@ struct Plan {
     size_t l2_chunk_bytes = 0;          // PHASTFT_L2_CHUNK_MB: signal bytes per chunk of a batched multi-pass call
     size_t pipe_ring_bytes = 0;         // PHASTFT_PIPE_RING_MB: workspace ring of the pipelined launch
     bool pipe_discard = true;           // PHASTFT_PIPE_DISCARD=0 keeps the ring's lines in L2 after pass 2 reads them
+    bool scribble_on = false;           // PHASTFT_SCRIBBLE=1: NaN-fill the workspace and staging before each use (scribble())
     std::string description;
 
     ~Plan() {
@@ -545,6 +569,7 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
         pl->pipe_ring_bytes = (size_t)std::max(1L, mb) << 20;
     }
     if (const char* e = getenv("PHASTFT_PIPE_DISCARD")) pl->pipe_discard = atoi(e) != 0;
+    pl->scribble_on = scribble_env();
     const bool il3 = pl->num_passes == 3 && pl->ws_il != 0;   // the middle pass reads and writes interleaved data
     // two-level W_N table
     pl->lo_bits = (ln + 1) / 2;
@@ -838,6 +863,7 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
         CUDA_TRY(cudaMalloc(&pl->ws_re, 2 * n * sizeof(T)));
         pl->ws_im = pl->ws_re + n;
         pl->ws_elems = n;
+        CUDA_TRY(scribble_new(pl->scribble_on, pl->ws_re, 2 * n * sizeof(T)));
     }
     if (pl->num_passes == 3) {
         // L2 blocking of passes 2+3: group size in bytes from PHASTFT_L2_GROUP_MB (default 32; 0 disables)
@@ -852,6 +878,8 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
             pl->l2_group = G;
             CUDA_TRY(cudaMalloc(&pl->ws2_re, (size_t)G * (n >> f[0]) * sizeof(T)));
             CUDA_TRY(cudaMalloc(&pl->ws2_im, (size_t)G * (n >> f[0]) * sizeof(T)));
+            CUDA_TRY(scribble_new(pl->scribble_on, pl->ws2_re, (size_t)G * (n >> f[0]) * sizeof(T)));
+            CUDA_TRY(scribble_new(pl->scribble_on, pl->ws2_im, (size_t)G * (n >> f[0]) * sizeof(T)));
         }
     }
     if (pl->num_passes == 2) {
@@ -1119,6 +1147,7 @@ int32_t grow_workspace(const Plan<T>& pl, size_t transforms, cudaStream_t stream
     CUDA_TRY(cudaMalloc(&pl.ws_re, 2 * transforms * pl.n * sizeof(T)));
     pl.ws_im = pl.ws_re + transforms * pl.n;
     pl.ws_elems = transforms * pl.n;
+    CUDA_TRY(scribble_new(pl.scribble_on, pl.ws_re, 2 * transforms * pl.n * sizeof(T)));
     return PHASTFT_OK;
 }
 
@@ -1247,9 +1276,22 @@ int32_t run_c2c(const Plan<T>& pl, const Io<T>& io, size_t batch, T scale, cudaS
             const size_t cap = std::max<size_t>(batch, 4096);
             CUDA_TRY(cudaMalloc(&pl.pipe_state, 64 + 2 * cap * sizeof(unsigned)));
             pl.pipe_state_batch = cap;
+            CUDA_TRY(scribble_new(pl.scribble_on, pl.pipe_state, 64 + 2 * cap * sizeof(unsigned)));
         }
     }
     if (!capturing && pl.ws_last_stream != stream && pl.ws_used) CUDA_TRY(cudaStreamWaitEvent(stream, pl.ws_free, 0));
+    // the part of the workspace this call uses: the pipelined launch's ring (both arrays in one run), else one chunk per array;
+    // the pipelined launch's state is zeroed below, the 3-pass group scratch is used whole
+    if (pipe) CUDA_TRY(scribble(pl.scribble_on, pl.ws_re, 2 * ring * pl.n * sizeof(T), stream));
+    else {
+        CUDA_TRY(scribble(pl.scribble_on, pl.ws_re, chunk * pl.n * sizeof(T), stream));
+        CUDA_TRY(scribble(pl.scribble_on, pl.ws_im, chunk * pl.n * sizeof(T), stream));
+    }
+    if (pl.num_passes == 3 && pl.ws2_re) {
+        const size_t g2 = (size_t)pl.l2_group * (pl.n >> pl.pass[0].log2R) * sizeof(T);
+        CUDA_TRY(scribble(pl.scribble_on, pl.ws2_re, g2, stream));
+        CUDA_TRY(scribble(pl.scribble_on, pl.ws2_im, g2, stream));
+    }
     const int P = pl.num_passes;
     if (pipe) {
         const bool lone = batch == 1;
@@ -1506,6 +1548,8 @@ int32_t fft_host(const Plan<T>* pl, T* re, size_t len_re, T* im, size_t len_im, 
         if (st) return st;
     }
     const size_t bytes = pl->n * sizeof(T);
+    CUDA_TRY(scribble(pl->scribble_on, pl->stage_re, bytes, pl->stream));
+    CUDA_TRY(scribble(pl->scribble_on, pl->stage_im, bytes, pl->stream));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, re, bytes, cudaMemcpyHostToDevice, pl->stream));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_im, im, bytes, cudaMemcpyHostToDevice, pl->stream));
     st = fft_dev(pl, pl->stage_re, pl->stage_im, direction, 1, pl->n, pl->stream);
@@ -1529,6 +1573,7 @@ int32_t fft_interleaved_host(const Plan<T>* pl, T* sig, size_t len_complex, int 
         if (st) return st;
     }
     const size_t bytes = 2 * pl->n * sizeof(T);
+    CUDA_TRY(scribble(pl->scribble_on, pl->stage_re, bytes, pl->stream));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, sig, bytes, cudaMemcpyHostToDevice, pl->stream));
     st = fft_interleaved_dev(pl, pl->stage_re, direction, 1, pl->n, pl->stream);
     if (st) return st;
@@ -1643,6 +1688,9 @@ int32_t batch_sharded_host(Plan<T>* const* plans, int num_plans, T* re, T* im, s
         }
         s.ev = true;
         if (!ev_ok) { (void)cudaGetLastError(); cleanup(); return fail(PHASTFT_ERR_CUDA, "cudaEventCreate"); }
+        const size_t staged = std::min<size_t>(NSLOT, s.chunks) * s.slot_elems * sizeof(T);
+        if (scribble(s.pl->scribble_on, s.pl->stage_re, staged, s.pl->stream_h2d) != cudaSuccess ||
+            scribble(s.pl->scribble_on, s.pl->stage_im, staged, s.pl->stream_h2d) != cudaSuccess) { (void)cudaGetLastError(); cleanup(); return fail(PHASTFT_ERR_CUDA, "cudaMemsetAsync"); }
     }
     // issue chunk j of every device before chunk j+1 of any, so all devices stream concurrently
     int32_t st = PHASTFT_OK;
@@ -1919,6 +1967,8 @@ int32_t build_plan_r2c(size_t n, int device, PlanR2c<T>** out) {
     CUDA_TRY(cudaMalloc(&pl->d_scr_re, (n / 2) * sizeof(T)));
     CUDA_TRY(cudaMalloc(&pl->d_scr_im, (n / 2) * sizeof(T)));
     pl->scr_elems = n / 2;
+    CUDA_TRY(scribble_new(pl->inner->scribble_on, pl->d_scr_re, (n / 2) * sizeof(T)));
+    CUDA_TRY(scribble_new(pl->inner->scribble_on, pl->d_scr_im, (n / 2) * sizeof(T)));
     CUDA_TRY(cudaEventCreateWithFlags(&pl->scr_free, cudaEventDisableTiming));
     *out = pl.release();
     return PHASTFT_OK;
@@ -2082,6 +2132,8 @@ int32_t c2r_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, T* d_out, 
         CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
         capturing = cap != cudaStreamCaptureStatusNone;
         if (!capturing && pl->scr_used && pl->scr_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, pl->scr_free, 0));
+        CUDA_TRY(scribble(in.scribble_on, d_sre, half * sizeof(T), stream));
+        CUDA_TRY(scribble(in.scribble_on, d_sim, half * sizeof(T), stream));
     }
     // (1) pre-process into scratch (r2c.rs:764-780)
     RealParams<T> rp;
@@ -2118,6 +2170,8 @@ int32_t grow_r2c_scratch(const PlanR2c<T>* pl, size_t elems) {
     cudaFree(pl->d_scr_re);
     cudaFree(pl->d_scr_im);
     pl->d_scr_re = re; pl->d_scr_im = im; pl->scr_elems = elems;
+    CUDA_TRY(scribble_new(pl->inner->scribble_on, re, elems * sizeof(T)));
+    CUDA_TRY(scribble_new(pl->inner->scribble_on, im, elems * sizeof(T)));
     return PHASTFT_OK;
 }
 
@@ -2191,6 +2245,8 @@ int32_t c2r_batch_dev(const PlanR2c<T>* pl, const T* d_ire, const T* d_iim, size
         d_sre = pl->d_scr_re; d_sim = pl->d_scr_im;
         own_scratch = true;
         if (!capturing && pl->scr_used && pl->scr_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, pl->scr_free, 0));
+        CUDA_TRY(scribble(pl->inner->scribble_on, d_sre, batch * half * sizeof(T), stream));
+        CUDA_TRY(scribble(pl->inner->scribble_on, d_sim, batch * half * sizeof(T), stream));
     }
     RealParams<T> rp;
     memset(&rp, 0, sizeof(rp));
@@ -2243,6 +2299,9 @@ int32_t r2c_host(const PlanR2c<T>* pl, const T* in, size_t len_in, T* ore, size_
     int32_t st = ensure_r2c_staging(pl);
     if (st) return st;
     cudaStream_t s = pl->inner->stream;
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_real, n * sizeof(T), s));
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_spec_re, (half + 1) * sizeof(T), s));
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_spec_im, (half + 1) * sizeof(T), s));
     CUDA_TRY(cudaMemcpyAsync(pl->d_real, in, n * sizeof(T), cudaMemcpyHostToDevice, s));
     st = r2c_dev(pl, pl->d_real, pl->d_spec_re, pl->d_spec_im, s);
     if (st) return st;
@@ -2274,6 +2333,9 @@ int32_t c2r_host(const PlanR2c<T>* pl, const T* ire, size_t len_ire, const T* ii
         int32_t st = ensure_r2c_staging(pl);
         if (st) return st;
     }
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_real, n * sizeof(T), s));
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_spec_re, (half + 1) * sizeof(T), s));
+    CUDA_TRY(scribble(pl->inner->scribble_on, pl->d_spec_im, (half + 1) * sizeof(T), s));
     CUDA_TRY(cudaMemcpyAsync(pl->d_spec_re, ire, (half + 1) * sizeof(T), cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(pl->d_spec_im, iim, (half + 1) * sizeof(T), cudaMemcpyHostToDevice, s));
     int32_t st = c2r_dev<T>(pl, pl->d_spec_re, pl->d_spec_im, pl->d_real, nullptr, nullptr, s);
@@ -2316,9 +2378,12 @@ struct AnyWorkspace {
     cudaEvent_t free_ev = nullptr;     // orders workspace reuse across streams (like Plan::ws_free)
     cudaStream_t last_stream = nullptr;
     bool used = false;
+    bool scribble_on = false;          // PHASTFT_SCRIBBLE=1, read when the plan is built: also covers the owner's host staging
     int32_t init(size_t e) {
+        scribble_on = scribble_env();
         CUDA_TRY(cudaMalloc(&ws, e * sizeof(cx<T>)));
         elems = e;
+        CUDA_TRY(scribble_new(scribble_on, ws, e * sizeof(cx<T>)));
         CUDA_TRY(cudaEventCreateWithFlags(&free_ev, cudaEventDisableTiming));
         return PHASTFT_OK;
     }
@@ -2338,6 +2403,7 @@ struct AnyWorkspace {
         CUDA_TRY(cudaDeviceSynchronize());   // every earlier user of the old workspace, on any stream, is done
         cudaFree(ws);
         ws = w; elems = e;
+        CUDA_TRY(scribble_new(scribble_on, ws, e * sizeof(cx<T>)));
         return PHASTFT_OK;
     }
     // Before a call's first launch (caller holds mu): room for `e` values, and the previous user on another stream is done.
@@ -2353,6 +2419,7 @@ struct AnyWorkspace {
             if (int32_t st = grow(e, members)) return st;
         }
         if (!capturing && used && last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, free_ev, 0));
+        CUDA_TRY(scribble(scribble_on, ws, e * sizeof(cx<T>), stream));
         return PHASTFT_OK;
     }
     // After a call's last launch.
@@ -2993,6 +3060,8 @@ int32_t any_host(const PlanAny<T>* pl, T* re, size_t len_re, T* im, size_t len_i
     }
     cudaStream_t s = pl->host_stream();
     const size_t bytes = pl->n * sizeof(T);
+    CUDA_TRY(scribble(pl->workspace().scribble_on, pl->stage_re, bytes, s));
+    CUDA_TRY(scribble(pl->workspace().scribble_on, pl->stage_im, bytes, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, re, bytes, cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_im, im, bytes, cudaMemcpyHostToDevice, s));
     if (int32_t st = any_dev(pl, pl->stage_re, pl->stage_im, direction, 1, pl->n, s)) return st;
@@ -3019,6 +3088,7 @@ int32_t any_interleaved_host(const PlanAny<T>* pl, T* sig, size_t len_complex, i
     }
     cudaStream_t s = pl->host_stream();
     const size_t bytes = 2 * pl->n * sizeof(T);
+    CUDA_TRY(scribble(pl->workspace().scribble_on, pl->stage_il, bytes, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_il, sig, bytes, cudaMemcpyHostToDevice, s));
     if (int32_t st = any_interleaved_dev(pl, pl->stage_il, direction, 1, pl->n, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(sig, pl->stage_il, bytes, cudaMemcpyDeviceToHost, s));
@@ -3206,13 +3276,17 @@ int32_t r2c_any_reserve(const PlanR2cAny<T>* pl, size_t batch) {
     return bluestein_reserve(pl->bs, batch);
 }
 
-// Caller holds host_mu.
+// Caller holds host_mu.  Under PHASTFT_SCRIBBLE=1 the staging is poisoned on `s` before the call's copies.
 template <typename T>
-int32_t ensure_r2c_any_staging(const PlanR2cAny<T>* pl) {
+int32_t ensure_r2c_any_staging(const PlanR2cAny<T>* pl, cudaStream_t s) {
     std::lock_guard<std::mutex> lock(pl->workspace().mu);   // released before the device call, which takes it
     if (!pl->stage_real) CUDA_TRY(cudaMalloc(&pl->stage_real, pl->n * sizeof(T)));
     if (!pl->stage_re) CUDA_TRY(cudaMalloc(&pl->stage_re, (pl->n / 2 + 1) * sizeof(T)));
     if (!pl->stage_im) CUDA_TRY(cudaMalloc(&pl->stage_im, (pl->n / 2 + 1) * sizeof(T)));
+    const bool on = pl->workspace().scribble_on;
+    CUDA_TRY(scribble(on, pl->stage_real, pl->n * sizeof(T), s));
+    CUDA_TRY(scribble(on, pl->stage_re, (pl->n / 2 + 1) * sizeof(T), s));
+    CUDA_TRY(scribble(on, pl->stage_im, (pl->n / 2 + 1) * sizeof(T), s));
     return PHASTFT_OK;
 }
 
@@ -3228,8 +3302,8 @@ int32_t r2c_any_host(const PlanR2cAny<T>* pl, const T* in, size_t len_in, T* ore
     if (!in || !ore || !oim) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> host_lock(pl->host_mu);
-    if (int32_t st = ensure_r2c_any_staging(pl)) return st;
     cudaStream_t s = pl->host_stream();
+    if (int32_t st = ensure_r2c_any_staging(pl, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(pl->stage_real, in, n * sizeof(T), cudaMemcpyHostToDevice, s));
     if (int32_t st = r2c_any_dev(pl, pl->stage_real, n, pl->stage_re, pl->stage_im, bins, 1, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(ore, pl->stage_re, bins * sizeof(T), cudaMemcpyDeviceToHost, s));
@@ -3249,8 +3323,8 @@ int32_t c2r_any_host(const PlanR2cAny<T>* pl, const T* ire, size_t len_ire, cons
     if (!ire || !iim || !out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> host_lock(pl->host_mu);
-    if (int32_t st = ensure_r2c_any_staging(pl)) return st;
     cudaStream_t s = pl->host_stream();
+    if (int32_t st = ensure_r2c_any_staging(pl, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(pl->stage_re, ire, bins * sizeof(T), cudaMemcpyHostToDevice, s));
     CUDA_TRY(cudaMemcpyAsync(pl->stage_im, iim, bins * sizeof(T), cudaMemcpyHostToDevice, s));
     if (int32_t st = c2r_any_dev(pl, pl->stage_re, pl->stage_im, bins, pl->stage_real, n, 1, s)) return st;
@@ -3295,6 +3369,7 @@ void phastft_oneshot_cache_clear(void) {
 }
 
 uint64_t phastft_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
+uint64_t phastft_last_scribble_bytes(void) { return g_scribble_bytes; }
 const char* phastft_last_launches(void) {
     std::string& s = g_launch_text;
     s.clear();
