@@ -90,6 +90,10 @@ template <> struct Api<double> {
     static int32_t c2r_any_dev(const R2cAny* p, const double* ire, const double* iim, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_any_f64_dev(p, ire, iim, is, out, os, b, s); }
     static int32_t r2c_any_host(const R2cAny* p, const double* in, std::size_t li, double* ore, std::size_t lre, double* oim, std::size_t lim) { return phastft_r2c_any_f64_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_any_host(const R2cAny* p, const double* ire, std::size_t lre, const double* iim, std::size_t lim, double* out, std::size_t lo) { return phastft_c2r_any_f64_host(p, ire, lre, iim, lim, out, lo); }
+    static int32_t r2c_il_dev(const R2cAny* p, const double* in, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_r2c_interleaved_any_f64_dev(p, in, is, out, os, b, s); }
+    static int32_t c2r_il_dev(const R2cAny* p, const double* in, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_interleaved_any_f64_dev(p, in, is, out, os, b, s); }
+    static int32_t r2c_il_host(const R2cAny* p, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_r2c_interleaved_any_f64_host(p, in, li, out, lo); }
+    static int32_t c2r_il_host(const R2cAny* p, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_c2r_interleaved_any_f64_host(p, in, li, out, lo); }
 };
 template <> struct Api<float> {
     using Dit = phastft_plan_dit_f32; using R2c = phastft_plan_r2c_f32;
@@ -131,6 +135,10 @@ template <> struct Api<float> {
     static int32_t c2r_any_dev(const R2cAny* p, const float* ire, const float* iim, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_any_f32_dev(p, ire, iim, is, out, os, b, s); }
     static int32_t r2c_any_host(const R2cAny* p, const float* in, std::size_t li, float* ore, std::size_t lre, float* oim, std::size_t lim) { return phastft_r2c_any_f32_host(p, in, li, ore, lre, oim, lim); }
     static int32_t c2r_any_host(const R2cAny* p, const float* ire, std::size_t lre, const float* iim, std::size_t lim, float* out, std::size_t lo) { return phastft_c2r_any_f32_host(p, ire, lre, iim, lim, out, lo); }
+    static int32_t r2c_il_dev(const R2cAny* p, const float* in, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_r2c_interleaved_any_f32_dev(p, in, is, out, os, b, s); }
+    static int32_t c2r_il_dev(const R2cAny* p, const float* in, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_interleaved_any_f32_dev(p, in, is, out, os, b, s); }
+    static int32_t r2c_il_host(const R2cAny* p, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_r2c_interleaved_any_f32_host(p, in, li, out, lo); }
+    static int32_t c2r_il_host(const R2cAny* p, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_c2r_interleaved_any_f32_host(p, in, li, out, lo); }
 };
 
 /// planner.rs:34-114
@@ -261,6 +269,24 @@ class PlannerR2cAny {
     void c2r_batch_dev(const T* d_in_re, const T* d_in_im, std::size_t in_stride, T* d_out, std::size_t out_stride, std::size_t batch,
                        void* stream = nullptr) const {
         check(Api<T>::c2r_any_dev(raw_, d_in_re, d_in_im, in_stride, d_out, out_stride, batch, stream));
+    }
+    /// r2c() with the N/2 + 1 bins as one interleaved host vector (its size the length checked); the planar call's results
+    void r2c_interleaved(const std::vector<T>& input, std::vector<std::complex<T>>& output) const {
+        check(Api<T>::r2c_il_host(raw_, input.data(), input.size(), reinterpret_cast<T*>(output.data()), output.size()));
+    }
+    /// c2r() from one interleaved host vector of N/2 + 1 bins
+    void c2r_interleaved(const std::vector<std::complex<T>>& input, std::vector<T>& output) const {
+        check(Api<T>::c2r_il_host(raw_, reinterpret_cast<const T*>(input.data()), input.size(), output.data(), output.size()));
+    }
+    /// `batch` r2c transforms on device pointers, member b at b * in_stride reals / complex element b * out_stride
+    void r2c_interleaved_device(const T* d_in, std::size_t in_stride, std::complex<T>* d_out, std::size_t out_stride, std::size_t batch,
+                                void* stream = nullptr) const {
+        check(Api<T>::r2c_il_dev(raw_, d_in, in_stride, reinterpret_cast<T*>(d_out), out_stride, batch, stream));
+    }
+    /// `batch` c2r transforms on device pointers, member b at complex element b * in_stride / b * out_stride reals
+    void c2r_interleaved_device(const std::complex<T>* d_in, std::size_t in_stride, T* d_out, std::size_t out_stride, std::size_t batch,
+                                void* stream = nullptr) const {
+        check(Api<T>::c2r_il_dev(raw_, reinterpret_cast<const T*>(d_in), in_stride, d_out, out_stride, batch, stream));
     }
   private:
     typename Api<T>::R2cAny* raw_ = nullptr;

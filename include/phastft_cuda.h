@@ -52,8 +52,11 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * for the register kernel or tile for the shared-memory one), SMOOTH-PRE-R2C / SMOOTH-PRE-C2R and ODD-R2C / ODD-C2R (the same with
  * the real any-length transforms' loads and last-pass stores), SMOOTH-POST-R2C (their halved r2c's untangle: R=<L>,
  * C=<members>) and CHIRP-PRE-IL / CHIRP-POST-IL / SMOOTH-PRE-IL / ODD-IL (the complex any-length transform's end kernels, the
- * last ODD pass only, in phastft_fft_interleaved_any_*: R, C and NT as in the planar call); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
- * copies), c2r-in (c2r pre-processing on load), cluster, pipe or pipe-tma; " pdl" marks programmatic dependent launch.
+ * last ODD pass only, in phastft_fft_interleaved_any_*: R, C and NT as in the planar call), R2C-UNTANGLE-IL / C2R-PRE-IL /
+ * CHIRP-POST-R2C-IL / CHIRP-PRE-C2R-IL / SMOOTH-PRE-C2R-IL / ODD-R2C-IL / SMOOTH-POST-R2C-IL (the spectrum's end of
+ * phastft_{r2c,c2r}_interleaved_any_*, whose halved mixed r2c's last pass is ODD-IL); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * copies), c2r-in (c2r pre-processing on load), c2r-in-il (the same from interleaved bins), cluster, pipe or pipe-tma; " pdl" marks
+ * programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
 PHASTFT_API const char* phastft_last_launches(void);
 /* Thread-local, like phastft_last_launches: the bytes of plan-owned scratch (workspaces, c2r scratch, host staging) that the
@@ -418,6 +421,34 @@ PHASTFT_API int32_t phastft_c2r_any_f64_host(const phastft_plan_r2c_any_f64* pla
                                              const double* in_im, size_t len_iim, double* output, size_t len_out);
 PHASTFT_API int32_t phastft_c2r_any_f32_host(const phastft_plan_r2c_any_f32* plan, const float* in_re, size_t len_ire,
                                              const float* in_im, size_t len_iim, float* output, size_t len_out);
+/* The same transforms with the spectrum as floor(n/2) + 1 interleaved (re, im) values (torch.fft.rfft / irfft(n=n),
+ * std::complex<T>, num_complex::Complex<T>): member b's bins start at complex element b * stride_complex of d_out / d_in
+ * (>= floor(n/2) + 1), a pointer aligned to 2 * sizeof(T) (a member may start at an odd complex offset); the real side keeps the
+ * rules above.  Forward unscaled, c2r scaled by 1/n, c2r never writes its input and drops Im X[0] for odd n, as the planar calls.
+ * Every path runs the planar call's launches with the spectrum's end kernels in interleaved modes (the power of two's last pass
+ * stores Z interleaved, then R2C-UNTANGLE-IL; its c2r reads the bins in the first pass (launch mode c2r-in-il) or in C2R-PRE-IL;
+ * CHIRP-POST-R2C-IL / CHIRP-PRE-C2R-IL; ODD-IL + SMOOTH-POST-R2C-IL, ODD-R2C-IL, SMOOTH-PRE-C2R-IL) and gives the planar call's
+ * results bit for bit.  NULL or misaligned pointers and short or odd strides return PHASTFT_ERR_INVALID_ARG before any launch;
+ * batch == 0, workspace growth, reserve() and graph capture as in the planar calls.  The host forms use the planar host length
+ * codes (r2c: input PHASTFT_ERR_INPUT_LEN, spectrum PHASTFT_ERR_OUTPUT_RE_LEN; c2r: spectrum PHASTFT_ERR_INPUT_RE_LEN, output
+ * PHASTFT_ERR_OUTPUT_LEN, lengths of the spectrum in complex values) and stage through a plan-owned buffer their first call
+ * allocates. */
+PHASTFT_API int32_t phastft_r2c_interleaved_any_f64_dev(const phastft_plan_r2c_any_f64* plan, const double* d_input, size_t in_stride,
+                                                        double* d_out, size_t out_stride_complex, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_r2c_interleaved_any_f32_dev(const phastft_plan_r2c_any_f32* plan, const float* d_input, size_t in_stride,
+                                                        float* d_out, size_t out_stride_complex, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_c2r_interleaved_any_f64_dev(const phastft_plan_r2c_any_f64* plan, const double* d_in, size_t in_stride_complex,
+                                                        double* d_output, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_c2r_interleaved_any_f32_dev(const phastft_plan_r2c_any_f32* plan, const float* d_in, size_t in_stride_complex,
+                                                        float* d_output, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_r2c_interleaved_any_f64_host(const phastft_plan_r2c_any_f64* plan, const double* input, size_t len_in,
+                                                         double* out, size_t len_out_complex);
+PHASTFT_API int32_t phastft_r2c_interleaved_any_f32_host(const phastft_plan_r2c_any_f32* plan, const float* input, size_t len_in,
+                                                         float* out, size_t len_out_complex);
+PHASTFT_API int32_t phastft_c2r_interleaved_any_f64_host(const phastft_plan_r2c_any_f64* plan, const double* in, size_t len_in_complex,
+                                                         double* output, size_t len_out);
+PHASTFT_API int32_t phastft_c2r_interleaved_any_f32_host(const phastft_plan_r2c_any_f32* plan, const float* in, size_t len_in_complex,
+                                                         float* output, size_t len_out);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

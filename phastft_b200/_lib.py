@@ -127,6 +127,10 @@ SIGNATURES = {
     "phastft_c2r_any_{s}_dev": ([_vp, _vp, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
     "phastft_r2c_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
     "phastft_c2r_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
+    "phastft_r2c_interleaved_any_{s}_dev": ([_vp, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_c2r_interleaved_any_{s}_dev": ([_vp, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_r2c_interleaved_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz], _i32),
+    "phastft_c2r_interleaved_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz], _i32),
 }
 def check(code: int):
     if code != OK:

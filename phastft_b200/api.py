@@ -43,6 +43,9 @@ __all__ = [
     "PlannerR2cAny64", "PlannerR2cAny32", "r2c_fft_f64_any_with_planner", "r2c_fft_f32_any_with_planner",
     "c2r_fft_f64_any_with_planner", "c2r_fft_f32_any_with_planner", "r2c_any_batch", "c2r_any_batch",
     "fft_64_interleaved_any_with_planner", "fft_32_interleaved_any_with_planner", "fft_interleaved_any_batch",
+    "r2c_fft_f64_interleaved_any_with_planner", "r2c_fft_f32_interleaved_any_with_planner",
+    "c2r_fft_f64_interleaved_any_with_planner", "c2r_fft_f32_interleaved_any_with_planner",
+    "r2c_interleaved_any_batch", "c2r_interleaved_any_batch",
 ]
 
 
@@ -778,9 +781,10 @@ def fft_any_batch(reals, imags, direction: Direction, planner, batch: int, batch
                                                       _torch_stream(reals)))
 
 
-def _complex_any_ptr(sfx, signal, planner, host):
-    """The pointer and length of an interleaved complex signal for planner (a PlannerAny of precision sfx): a torch CUDA
-    complex tensor, or with host=True also a numpy array.  Raises before anything reaches the library."""
+def _complex_any_ptr(sfx, signal, planner, host, writable=True):
+    """The pointer and length of an interleaved complex signal for planner (a PlannerAny or PlannerR2cAny of precision sfx): a
+    torch CUDA complex tensor, or with host=True also a numpy array (writable unless `writable` is False).  Raises before
+    anything reaches the library."""
     if planner._sfx != sfx:
         raise TypeError("planner precision does not match the function")
     if _is_torch(signal):
@@ -796,7 +800,7 @@ def _complex_any_ptr(sfx, signal, planner, host):
     cdtype = np.complex128 if sfx == "f64" else np.complex64
     if not isinstance(signal, np.ndarray) or signal.dtype != cdtype or signal.ndim != 1 or not signal.flags.c_contiguous:
         raise TypeError(f"expected a contiguous 1-D {np.dtype(cdtype)} array or a torch CUDA complex tensor")
-    if not signal.flags.writeable:
+    if writable and not signal.flags.writeable:
         raise ValueError("signal is read-only")
     return signal.ctypes.data_as(C.c_void_p), signal.size
 
@@ -940,3 +944,100 @@ def c2r_any_batch(in_re, in_im, out, planner, batch: int, in_stride: int | None 
     """c2r_batch for any length: member b reads N/2 + 1 bins at in_re / in_im[b * in_stride:] and writes N reals at
     out[b * out_stride:] (defaults: N/2 + 1 and N).  For even N the out-stride must be even (the output is written as pairs)."""
     _c2r_any(planner._sfx, in_re, in_im, out, planner, int(batch), in_stride, out_stride)
+
+
+# ----------------------------------------------------------------------------------------------
+# real-input FFTs of any length with the spectrum as interleaved complex bins (torch.fft.rfft / irfft's layout)
+# ----------------------------------------------------------------------------------------------
+def _r2c_interleaved_any(sfx, x, out, planner, batch, in_stride, out_stride):
+    po, no = _complex_any_ptr(sfx, out, planner, False)
+    n, bins = planner.n, planner.n // 2 + 1
+    in_stride = n if in_stride is None else int(in_stride)
+    out_stride = bins if out_stride is None else int(out_stride)
+    px, nx = _torch_ptr(x, planner._dtype)
+    _check_batch_len("input", nx, batch, in_stride, n)
+    _check_batch_len("output", no, batch, out_stride, bins)
+    if n % 2 == 0 and not _pair_aligned(x):                   # even n reads the input as pairs: an aligned copy
+        x = x.clone()
+        px = C.c_void_p(x.data_ptr())
+    check(fn("phastft_r2c_interleaved_any_{s}_dev", sfx)(planner._h, px, in_stride, po, out_stride, int(batch), _torch_stream(x)))
+
+
+def _c2r_interleaved_any(sfx, spec, out, planner, batch, in_stride, out_stride):
+    ps, ns = _complex_any_ptr(sfx, spec, planner, False)
+    n, bins = planner.n, planner.n // 2 + 1
+    in_stride = bins if in_stride is None else int(in_stride)
+    out_stride = n if out_stride is None else int(out_stride)
+    _, no = _torch_ptr(out, planner._dtype)
+    _check_batch_len("input", ns, batch, in_stride, bins)
+    _check_batch_len("output", no, batch, out_stride, n)
+    work = out if n % 2 or _pair_aligned(out) else out.clone()   # even n writes pairs; the clone keeps what lies between members
+    check(fn("phastft_c2r_interleaved_any_{s}_dev", sfx)(planner._h, ps, in_stride, C.c_void_p(work.data_ptr()), out_stride,
+                                                         int(batch), _torch_stream(out)))
+    if work is not out:
+        out.copy_(work)
+
+
+def _r2c_interleaved_any_with_planner(sfx, dtype, x, out, planner):
+    if _is_torch(x):
+        _, no = _complex_any_ptr(sfx, out, planner, False)
+        if x.numel() != planner.n:
+            raise PhastFTPanic(5)
+        if no != planner.n // 2 + 1:
+            raise PhastFTPanic(6)
+        _r2c_interleaved_any(sfx, x, out, planner, 1, None, None)
+    else:
+        if _is_torch(out):
+            raise TypeError("numpy input with a torch output: pass both as numpy arrays or both as torch CUDA tensors")
+        po, no = _complex_any_ptr(sfx, out, planner, True)
+        px, nx = _np_ptr(x, dtype, False)
+        check(fn("phastft_r2c_interleaved_any_{s}_host", sfx)(planner._h, px, nx, po, no))
+
+
+def _c2r_interleaved_any_with_planner(sfx, dtype, spec, out, planner):
+    if _is_torch(out):
+        _, ns = _complex_any_ptr(sfx, spec, planner, False)
+        if out.numel() != planner.n:
+            raise PhastFTPanic(8)
+        if ns != planner.n // 2 + 1:
+            raise PhastFTPanic(9)
+        _c2r_interleaved_any(sfx, spec, out, planner, 1, None, None)
+    else:
+        if _is_torch(spec):
+            raise TypeError("torch input with a numpy output: pass both as numpy arrays or both as torch CUDA tensors")
+        ps, ns = _complex_any_ptr(sfx, spec, planner, True, writable=False)
+        po, no = _np_ptr(out, dtype, True)
+        check(fn("phastft_c2r_interleaved_any_{s}_host", sfx)(planner._h, ps, ns, po, no))
+
+
+def r2c_fft_f64_interleaved_any_with_planner(input_re, output, planner: PlannerR2cAny64) -> None:
+    """r2c_fft_f64_any_with_planner with the N/2 + 1 bins (N/2 rounded down) as one complex128 array: a float64 / complex128 numpy
+    pair (synchronous) or torch CUDA tensors (torch's current stream), the layout of torch.fft.rfft.  Bit-identical to the planar
+    call on the same plan."""
+    _r2c_interleaved_any_with_planner("f64", np.float64, input_re, output, planner)
+
+
+def r2c_fft_f32_interleaved_any_with_planner(input_re, output, planner: PlannerR2cAny32) -> None:
+    _r2c_interleaved_any_with_planner("f32", np.float32, input_re, output, planner)
+
+
+def c2r_fft_f64_interleaved_any_with_planner(input, output, planner: PlannerR2cAny64) -> None:
+    """c2r_fft_f64_any_with_planner from N/2 + 1 complex128 bins (torch.fft.irfft(spec, n=N)'s input), normalised so that
+    c2r(r2c(x)) == x; the input is never written."""
+    _c2r_interleaved_any_with_planner("f64", np.float64, input, output, planner)
+
+
+def c2r_fft_f32_interleaved_any_with_planner(input, output, planner: PlannerR2cAny32) -> None:
+    _c2r_interleaved_any_with_planner("f32", np.float32, input, output, planner)
+
+
+def r2c_interleaved_any_batch(x, out, planner, batch: int, in_stride: int | None = None, out_stride: int | None = None) -> None:
+    """r2c_any_batch into a flat 1-D complex torch CUDA tensor: member b reads N reals at x[b * in_stride:] and writes N/2 + 1
+    bins at out[b * out_stride:] (complex values; defaults: N and N/2 + 1)."""
+    _r2c_interleaved_any(planner._sfx, x, out, planner, int(batch), in_stride, out_stride)
+
+
+def c2r_interleaved_any_batch(spec, out, planner, batch: int, in_stride: int | None = None, out_stride: int | None = None) -> None:
+    """c2r_any_batch from a flat 1-D complex torch CUDA tensor: member b reads N/2 + 1 bins at spec[b * in_stride:] (complex
+    values) and writes N reals at out[b * out_stride:] (defaults: N/2 + 1 and N)."""
+    _c2r_interleaved_any(planner._sfx, spec, out, planner, int(batch), in_stride, out_stride)

@@ -184,7 +184,10 @@ __device__ __forceinline__ void bulk_load_1d(unsigned smem_dst, const void* gsrc
 //      last stage writes its results into a second planar staging area and two cp.async.bulk copies take them out.  The
 //      per-lane 4/8-byte accesses of the plain kernel (128 bytes per f32 warp instruction, the bound of the 16..128-point
 //      batches) become two asynchronous copies per CTA.
-enum { MODE_PLAIN = 0, MODE_XCH_PRODUCE = 1, MODE_XCH_CONSUME = 2, MODE_TMA_IN = 3, MODE_BULK_IN = 4, MODE_C2R_IN = 5, MODE_ROW_BULK = 6 };
+//   7  as 5 with the half-spectrum's bins interleaved (phastft_c2r_interleaved_any_*): in_re holds N/2 + 1 Complex<T> values
+//      per member and bins k and N/2 - k are one Complex<T> load each; the arithmetic is mode 5's
+enum { MODE_PLAIN = 0, MODE_XCH_PRODUCE = 1, MODE_XCH_CONSUME = 2, MODE_TMA_IN = 3, MODE_BULK_IN = 4, MODE_C2R_IN = 5, MODE_ROW_BULK = 6,
+       MODE_C2R_IN_IL = 7 };
 template <typename T, class RL, int C, int NT, int KIND, int XCH = 0, int VARIANT = 0>
 struct PassKernel {
     static constexpr int S = RL::S;
@@ -199,6 +202,7 @@ struct PassKernel {
     static constexpr int TILE_ELEMS = (S >= 2) ? R * C : 0;
     static constexpr int G_ELEMS = (KIND == KIND_TRANS) ? C * R1 : R1;
     static constexpr bool ASYNC_IN = (XCH == MODE_TMA_IN || XCH == MODE_BULK_IN || XCH == MODE_ROW_BULK);
+    static constexpr bool C2R_IN = (XCH == MODE_C2R_IN || XCH == MODE_C2R_IN_IL);   // c2r pre-processing on load
     // strided tiles whose last stage is radix 32 (1024 = 32 x 32, 512 = 16 x 32): that stage reads W_R^(m*i) from the plan's
     // [m][i] table (PassParams::tw_stage_im), and stage 1 is written as a single trip when it can be (see body())
     static constexpr bool STAGE32 = KIND != KIND_ROW && S >= 2 && RL::rad(S - 1) == 32;
@@ -244,6 +248,7 @@ struct PassKernel {
     // (same arithmetic, in the same order, as c2r_preprocess_kernel below; r2c.rs:263-347).  The inverse runs as a forward
     // transform of the swapped parts (r2c.rs:782), so the kernel is handed (im, re).
     // `mbase`: where the batch member's spectrum starts (member * in_bstride); a0 - mbase is the bin index.
+    // MODE_C2R_IN_IL: the same bins as one Complex<T> each (indices and strides count complex values).
     template <int N>
     static __device__ __forceinline__ void gload_c2r(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N],
                                                      long long mbase) {
@@ -257,6 +262,8 @@ struct PassKernel {
         const T* __restrict__ fi = p.in_im + a0;
         const T* __restrict__ sr = p.in_re + (mbase + half - k0);
         const T* __restrict__ si = p.in_im + (mbase + half - k0);
+        [[maybe_unused]] const cx<T>* __restrict__ fc = reinterpret_cast<const cx<T>*>(p.in_re) + a0;
+        [[maybe_unused]] const cx<T>* __restrict__ sc = reinterpret_cast<const cx<T>*>(p.in_re) + (mbase + half - k0);
         const double2 wb = p.pre_tw2.get((uint32_t)k0);
         constexpr int G = (sizeof(T) == 8 && N > 8) ? 8 : N;
 #pragma unroll
@@ -265,8 +272,14 @@ struct PassKernel {
 #pragma unroll
             for (int i = 0; i < G; ++i) {
                 const long long off = (long long)(g0 + i) * step;
-                re_f[i] = fr[off]; im_f[i] = fi[off];
-                re_s[i] = sr[-off]; im_s[i] = -si[-off];
+                if constexpr (XCH == MODE_C2R_IN_IL) {
+                    const cx<T> f = fc[off], s = sc[-off];
+                    re_f[i] = f.x; im_f[i] = f.y;
+                    re_s[i] = s.x; im_s[i] = -s.y;
+                } else {
+                    re_f[i] = fr[off]; im_f[i] = fi[off];
+                    re_s[i] = sr[-off]; im_s[i] = -si[-off];
+                }
             }
 #pragma unroll
             for (int i = 0; i < G; ++i) {
@@ -283,7 +296,7 @@ struct PassKernel {
     template <int N, int IL = -1>
     static __device__ __forceinline__ void gload_n(const PassParams<T>& p, long long a0, long long step, cx<T> (&x)[N],
                                                    [[maybe_unused]] long long mbase = 0) {
-        if constexpr (XCH == MODE_C2R_IN) {
+        if constexpr (C2R_IN) {
             gload_c2r<N>(p, a0, step, x, mbase);
         } else if constexpr (IL < 0) {
             if (p.in_interleaved == 0) gload_n<N, 0>(p, a0, step, x);
@@ -484,7 +497,7 @@ struct PassKernel {
         uint32_t kp0 = 0;              // previous-pass output digit of column c = 0
         uint32_t kp_cstep = 0;         // ... and its increment per column
         uint32_t bcol0 = 0;            // flat index of the remaining digits for column 0 (COL only)
-        [[maybe_unused]] long long mbase = 0;   // MODE_C2R_IN: first input element of this tile's batch member
+        [[maybe_unused]] long long mbase = 0;   // MODE_C2R_IN(_IL): first input element of this tile's batch member
 
         if constexpr (KIND == KIND_COL) {
             const int tilesB = 1 << (p.log2B - LOG2C);
@@ -495,7 +508,7 @@ struct PassKernel {
             const int batch = rest >> p.log2A;
             const long long off = ((long long)a << (LOG2R + p.log2B)) + ((long long)bt << LOG2C);
             in_base = (long long)batch * p.in_bstride + off;
-            if constexpr (XCH == MODE_C2R_IN) mbase = (long long)batch * p.in_bstride;
+            if constexpr (C2R_IN) mbase = (long long)batch * p.in_bstride;
             out_base = (long long)(p.out_ring ? (batch & (p.out_ring - 1)) : batch) * p.out_bstride + off;
             in_rstride = 1LL << p.log2B;
             in_cstride = 1;
@@ -712,7 +725,7 @@ struct PassKernel {
                 if constexpr (PRELOAD && STAGE32) break;
             }
         };
-        if constexpr (PRELOAD || XCH == MODE_C2R_IN) stage1(std::integral_constant<int, 0>{});
+        if constexpr (PRELOAD || C2R_IN) stage1(std::integral_constant<int, 0>{});
         else if (p.in_interleaved == 0) stage1(std::integral_constant<int, 0>{});
         else if (p.in_interleaved == 1) stage1(std::integral_constant<int, 1>{});
         else stage1(std::integral_constant<int, 2>{});
@@ -869,70 +882,96 @@ __global__ void __launch_bounds__(NTF, MINB) fft_pipe2_kernel(const __grid_const
 // CPU) is replaced by a two-level lookup: consecutive k hit consecutive `lo` entries (coalesced)
 // and one broadcast `hi` entry.
 // ---------------------------------------------------------------------------------------------
+// A member's spectrum bins: planar (re[k], im[k]), or SIL: Complex<T> values at re (im unused), as the interleaved real
+// transforms (phastft_{r2c,c2r}_interleaved_any_*) hold them.  One complex value per access: an interleaved f32 member may start
+// at an odd complex offset, so it is only 8-byte aligned.
+template <typename T, bool SIL>
+struct SpecBins {
+    T* re;
+    T* im;
+    __device__ __forceinline__ cx<T> get(long long k) const {
+        if constexpr (SIL) return reinterpret_cast<const cx<T>*>(re)[k];
+        else return make_cx<T>(re[k], im[k]);
+    }
+    __device__ __forceinline__ void put(long long k, T x, T y) const {
+        if constexpr (SIL) reinterpret_cast<cx<T>*>(re)[k] = make_cx<T>(x, y);
+        else { re[k] = x; im[k] = y; }
+    }
+};
+// the bins of the member `off` bins in (planar: elements of each array; SIL: complex values)
+template <typename T, bool SIL>
+__device__ __forceinline__ SpecBins<T, SIL> spec_at(const T* re, const T* im, long long off) {
+    if constexpr (SIL) return {const_cast<T*>(reinterpret_cast<const T*>(reinterpret_cast<const cx<T>*>(re) + off)), nullptr};
+    else return {const_cast<T*>(re + off), const_cast<T*>(im + off)};
+}
+
 template <typename T>
 struct RealParams {
     T* __restrict__ re;         // untangle: in/out (length half+1).  preprocess: z_re out (length half)
     T* __restrict__ im;
     const T* __restrict__ in_re;  // preprocess only: spectrum (length half+1)
     const T* __restrict__ in_im;
-    long long bstride;          // elements between batch members in re/im
-    long long in_bstride;
+    long long bstride;          // elements between batch members in re/im (the interleaved untangle: complex values)
+    long long in_bstride;       // (the interleaved preprocess: complex values)
     int log2half;
     unsigned blocks_per_member; // the grid is members x blocks_per_member blocks, member-major
     Tw2 tw2;                    // two-level table for W_N, N = 2*half
 };
 
-template <typename T>
+// SIL: the bins are interleaved (R2C-UNTANGLE-IL)
+template <typename T, bool SIL = false>
 __global__ void __launch_bounds__(256) r2c_untangle_kernel(const __grid_constant__ RealParams<T> p) {
     const long long half = 1LL << p.log2half;
     const long long q = half >> 1;
     const unsigned mb = blockIdx.x / p.blocks_per_member;
     const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * blockDim.x + threadIdx.x;
-    T* re = p.re + (long long)mb * p.bstride;
-    T* im = p.im + (long long)mb * p.bstride;
+    const SpecBins<T, SIL> y = spec_at<T, SIL>(p.re, p.im, (long long)mb * p.bstride);
     if (k > q) return;
     if (k == 0) {
         // r2c.rs:161-166
-        T a0 = re[0], b0 = im[0];
-        re[0] = a0 + b0; im[0] = T(0);
-        re[half] = a0 - b0; im[half] = T(0);
+        const cx<T> z0 = y.get(0);
+        T a0 = z0.x, b0 = z0.y;
+        y.put(0, a0 + b0, T(0));
+        y.put(half, a0 - b0, T(0));
         return;
     }
     double2 wd = p.tw2.get((uint32_t)k);
     const T wkr = T(0.5 * wd.x), wki = T(0.5 * wd.y);
     if (k == q) {
         // r2c.rs:233-236 (self pair)
-        T a = re[q], b = im[q];
-        re[q] = a + T(2) * wkr * b;
-        im[q] = T(2) * wki * b;
+        const cx<T> zq = y.get(q);
+        T a = zq.x, b = zq.y;
+        y.put(q, a + T(2) * wkr * b, T(2) * wki * b);
         return;
     }
     const long long m = half - k;
-    T a = re[k], b = im[k], c = re[m], d = im[m];
+    const cx<T> zk = y.get(k), zm = y.get(m);
+    T a = zk.x, b = zk.y, c = zm.x, d = zm.y;
     T s_re = T(0.5) * (a + c), s_im = T(0.5) * (b - d);
     T t_re = b + d, t_im = c - a;
     T wzr = wkr * t_re - wki * t_im;
     T wzi = wkr * t_im + wki * t_re;
-    re[k] = s_re + wzr; im[k] = s_im + wzi;
-    re[m] = s_re - wzr; im[m] = wzi - s_im;
+    y.put(k, s_re + wzr, s_im + wzi);
+    y.put(m, s_re - wzr, wzi - s_im);
 }
 
-template <typename T>
+// SIL: the spectrum is interleaved (C2R-PRE-IL); z stays planar
+template <typename T, bool SIL = false>
 __global__ void __launch_bounds__(256) c2r_preprocess_kernel(const __grid_constant__ RealParams<T> p) {
     const long long half = 1LL << p.log2half;
     const unsigned mb = blockIdx.x / p.blocks_per_member;
     const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * blockDim.x + threadIdx.x;
     if (k >= half) return;
-    const T* ire = p.in_re + (long long)mb * p.in_bstride;
-    const T* iim = p.in_im + (long long)mb * p.in_bstride;
+    const SpecBins<T, SIL> x = spec_at<T, SIL>(p.in_re, p.in_im, (long long)mb * p.in_bstride);
     T* zre = p.re + (long long)mb * p.bstride;
     T* zim = p.im + (long long)mb * p.bstride;
     const long long m = half - k;
     double2 wd = p.tw2.get((uint32_t)k);
     const T c_h = T(0.5 * wd.x), s_h = T(0.5 * wd.y);
     // r2c.rs:263-347
-    T re_f = ire[k], im_f = iim[k];
-    T re_s = ire[m], im_s = -iim[m];
+    const cx<T> xf = x.get(k), xs = x.get(m);
+    T re_f = xf.x, im_f = xf.y;
+    T re_s = xs.x, im_s = -xs.y;
     T zx_re = T(0.5) * (re_f + re_s), zx_im = T(0.5) * (im_f + im_s);
     T dr = re_f - re_s, di = im_f - im_s;
     T zy_re = c_h * dr + s_h * di;
@@ -991,7 +1030,20 @@ struct ChirpParams {
 //   C2R_DIRECT   bins 0 .. floor(N/2) in, the Hermitian extension (swapped); the real part of the inverse out
 //   C2C_IL       interleaved complex in and out (phastft_fft_interleaved_any_*), the forward direction
 //   C2C_IL_SWAP  the same for the reverse direction: re / im swapped on load and on store, as the planar call swaps its pointers
-enum ChirpMode { CHIRP_C2C, CHIRP_R2C_HALVED, CHIRP_R2C_DIRECT, CHIRP_C2R_HALVED, CHIRP_C2R_DIRECT, CHIRP_C2C_IL, CHIRP_C2C_IL_SWAP };
+//   R2C_HALVED_IL, R2C_DIRECT_IL, C2R_HALVED_IL, C2R_DIRECT_IL  the real modes with the spectrum as interleaved Complex<T> bins
+//                (phastft_{r2c,c2r}_interleaved_any_*): only the spectrum's end runs them (CHIRP-POST of r2c, CHIRP-PRE of c2r);
+//                the real side runs the planar mode's kernel
+enum ChirpMode { CHIRP_C2C, CHIRP_R2C_HALVED, CHIRP_R2C_DIRECT, CHIRP_C2R_HALVED, CHIRP_C2R_DIRECT, CHIRP_C2C_IL, CHIRP_C2C_IL_SWAP,
+                 CHIRP_R2C_HALVED_IL, CHIRP_R2C_DIRECT_IL, CHIRP_C2R_HALVED_IL, CHIRP_C2R_DIRECT_IL };
+
+// a real mode with an interleaved spectrum, and the planar mode whose arithmetic it runs (the mode itself for the others)
+template <int MODE>
+__host__ __device__ constexpr bool chirp_spec_il() { return MODE >= CHIRP_R2C_HALVED_IL; }
+template <int MODE>
+__host__ __device__ constexpr int chirp_planar() {
+    return MODE == CHIRP_R2C_HALVED_IL ? CHIRP_R2C_HALVED : MODE == CHIRP_R2C_DIRECT_IL ? CHIRP_R2C_DIRECT
+         : MODE == CHIRP_C2R_HALVED_IL ? CHIRP_C2R_HALVED : MODE == CHIRP_C2R_DIRECT_IL ? CHIRP_C2R_DIRECT : MODE;
+}
 
 // The interleaved modes' ends.  The swap is part of the mode, so no kernel carries a runtime test for it.  The caller's array is
 // accessed one complex value at a time: a member starts at any complex offset, so f32 members are only 8-byte aligned.
@@ -1012,7 +1064,7 @@ __device__ __forceinline__ cx<T> il_store(const cx<T>& v, T scale) {
 // CHIRP-POST's items per member: values, or bin pairs (k, L - k) for R2C_HALVED
 template <int MODE>
 __host__ __device__ constexpr long long chirp_post_count(long long n) {
-    return MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT ? n / 2 + 1 : n;
+    return chirp_planar<MODE>() == CHIRP_R2C_HALVED || chirp_planar<MODE>() == CHIRP_R2C_DIRECT ? n / 2 + 1 : n;
 }
 
 // W_N^k for 0 <= k < L, N = 2L, from the table of k <= L/2: W_N^k = -conj(W_N^(L-k))
@@ -1024,13 +1076,14 @@ __device__ __forceinline__ cx<T> chirp_wn(const ChirpParams<T>& p, long long k) 
 }
 
 // The real modes' arithmetic at the two ends, shared by the Bluestein (CHIRP-*) and mixed-radix (SMOOTH-* / ODD) kernels.
-// c2r_preprocess_kernel's formula with w = W_N^m, L = N/2 bins in re / im: z = (X[m] + conj X[L-m]) / 2 +
+// c2r_preprocess_kernel's formula with w = W_N^m, L = N/2 bins x: z = (X[m] + conj X[L-m]) / 2 +
 // i conj(w) (X[m] - conj X[L-m]) / 2, swapped for the inverse
-template <typename T>
-__device__ __forceinline__ cx<T> c2r_halved_in(const T* re, const T* im, long long l, long long m, cx<T> w) {
+template <typename T, bool SIL>
+__device__ __forceinline__ cx<T> c2r_halved_in(const SpecBins<T, SIL>& x, long long l, long long m, cx<T> w) {
     const long long s = l - m;
     const T c_h = T(0.5) * w.x, s_h = T(0.5) * w.y;
-    const T re_f = re[m], im_f = im[m], re_s = re[s], im_s = -im[s];
+    const cx<T> xf = x.get(m), xs = x.get(s);
+    const T re_f = xf.x, im_f = xf.y, re_s = xs.x, im_s = -xs.y;
     const T zx_re = T(0.5) * (re_f + re_s), zx_im = T(0.5) * (im_f + im_s);
     const T dr = re_f - re_s, di = im_f - im_s;
     const T zy_re = c_h * dr + s_h * di;
@@ -1038,9 +1091,14 @@ __device__ __forceinline__ cx<T> c2r_halved_in(const T* re, const T* im, long lo
     return make_cx<T>(zx_im + zy_re, zx_re - zy_im);
 }
 // odd N: the Hermitian extension Y[m] = X[m] (m <= N/2) or conj X[N - m], swapped
-template <typename T>
-__device__ __forceinline__ cx<T> c2r_direct_in(const T* re, const T* im, long long n, long long m) {
-    return 2 * m <= n ? make_cx<T>(im[m], re[m]) : make_cx<T>(-im[n - m], re[n - m]);
+template <typename T, bool SIL>
+__device__ __forceinline__ cx<T> c2r_direct_in(const SpecBins<T, SIL>& x, long long n, long long m) {
+    if constexpr (SIL) {
+        const cx<T> v = x.get(2 * m <= n ? m : n - m);
+        return 2 * m <= n ? make_cx<T>(v.y, v.x) : make_cx<T>(-v.y, v.x);
+    } else {
+        return 2 * m <= n ? make_cx<T>(x.im[m], x.re[m]) : make_cx<T>(-x.im[n - m], x.re[n - m]);
+    }
 }
 // r2c_untangle_kernel's formula for the bin pair (k, L - k) of Z = DFT_L(z), w = W_N^k: X[k] and X[L - k]
 template <typename T>
@@ -1058,13 +1116,15 @@ __device__ __forceinline__ void r2c_untangle(cx<T> zk, cx<T> zm, cx<T> w, cx<T>&
 // CHIRP-PRE's value before the chirp product, real modes: member mb's element m < L
 template <typename T, int MODE>
 __device__ __forceinline__ cx<T> chirp_real_in(const ChirpParams<T>& p, unsigned mb, long long m) {
+    constexpr int PM = chirp_planar<MODE>();
     const T* re = p.in_re + (long long)mb * p.bstride;
-    if constexpr (MODE == CHIRP_R2C_HALVED) {
+    if constexpr (PM == CHIRP_R2C_HALVED) {
         return reinterpret_cast<const cx<T>*>(re)[m];                   // (x[2m], x[2m+1]): base and stride keep pairs aligned
     } else {
-        const T* im = p.in_im + (long long)mb * p.bstride;
-        if constexpr (MODE == CHIRP_C2R_HALVED) return c2r_halved_in<T>(re, im, p.n, m, chirp_wn(p, m));
-        else return c2r_direct_in<T>(re, im, p.n, m);
+        // bstride counts T either way: the interleaved spectrum's member starts at re
+        const SpecBins<T, chirp_spec_il<MODE>()> x = spec_at<T, chirp_spec_il<MODE>()>(re, p.in_im + (long long)mb * p.bstride, 0);
+        if constexpr (PM == CHIRP_C2R_HALVED) return c2r_halved_in<T>(x, p.n, m, chirp_wn(p, m));
+        else return c2r_direct_in<T>(x, p.n, m);
     }
 }
 
@@ -1092,7 +1152,7 @@ __global__ void __launch_bounds__(256) chirp_pre_kernel(const __grid_constant__ 
 #pragma unroll
             for (int j = 0; j < P::V; ++j)
                 a[j] = m0 + j < p.n ? cmul<T>(make_cx<T>(re[m0 + j], im[m0 + j]), w[j]) : make_cx<T>(T(0), T(0));
-        } else if constexpr (MODE == CHIRP_R2C_DIRECT) {
+        } else if constexpr (chirp_planar<MODE>() == CHIRP_R2C_DIRECT) {
             const T* re = p.in_re + (long long)mb * p.bstride;            // real x complex: any element offset is legal
 #pragma unroll
             for (int j = 0; j < P::V; ++j) {
@@ -1162,11 +1222,12 @@ __global__ void __launch_bounds__(256) chirp_post_kernel(const __grid_constant__
             if (k0 + j >= p.n) break;
             y[k0 + j] = il_store<T, MODE>(cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y)), p.scale);
         }
-    } else if constexpr (MODE == CHIRP_R2C_HALVED) {
+    } else if constexpr (chirp_planar<MODE>() == CHIRP_R2C_HALVED) {
         // bin pair (k, L - k): Z[k] = w[k] conj C[k] and Z[L - k] (Z[L] = Z[0]), then r2c_untangle_kernel's formula with W_N^k;
         // k = 0 gives X[0] and X[L] = X[N/2], k = L/2 (L even) is the self pair.  The mirrored reads are one value each.
-        T* re = p.out_re + (long long)mb * p.out_bstride;
-        T* im = p.out_im + (long long)mb * p.out_bstride;
+        // out_bstride counts T either way.
+        const SpecBins<T, chirp_spec_il<MODE>()> y =
+            spec_at<T, chirp_spec_il<MODE>()>(p.out_re + (long long)mb * p.out_bstride, p.out_im + (long long)mb * p.out_bstride, 0);
 #pragma unroll
         for (int j = 0; j < P::V; ++j) {
             const long long k = k0 + j;
@@ -1177,18 +1238,17 @@ __global__ void __launch_bounds__(256) chirp_post_kernel(const __grid_constant__
             const cx<T> zm = cmul<T>(wm, make_cx<T>(cm.x, -cm.y));
             cx<T> xk, xm;
             r2c_untangle<T>(zk, zm, p.wn[k], xk, xm);
-            re[k] = xk.x; im[k] = xk.y;
-            if (m != k) { re[m] = xm.x; im[m] = xm.y; }
+            y.put(k, xk.x, xk.y);
+            if (m != k) y.put(m, xm.x, xm.y);
         }
-    } else if constexpr (MODE == CHIRP_R2C_DIRECT) {
-        T* re = p.out_re + (long long)mb * p.out_bstride;
-        T* im = p.out_im + (long long)mb * p.out_bstride;
+    } else if constexpr (chirp_planar<MODE>() == CHIRP_R2C_DIRECT) {
+        const SpecBins<T, chirp_spec_il<MODE>()> y =
+            spec_at<T, chirp_spec_il<MODE>()>(p.out_re + (long long)mb * p.out_bstride, p.out_im + (long long)mb * p.out_bstride, 0);
 #pragma unroll
         for (int j = 0; j < P::V; ++j) {
             if (k0 + j >= count) break;
             const cx<T> x = cmul<T>(w[j], make_cx<T>(c[j].x, -c[j].y));
-            re[k0 + j] = x.x;
-            im[k0 + j] = x.y;
+            y.put(k0 + j, x.x, x.y);
         }
     } else if constexpr (MODE == CHIRP_C2R_HALVED) {
         // y = swap(w conj C) / L, the pair (y[2k], y[2k+1]): one aligned 2 * sizeof(T) store
@@ -1251,7 +1311,8 @@ struct OddParams {
     const unsigned short* perm;    // tile kernel: where stage 1 puts the butterfly of row r < R / rad[0] (digit reversal)
     long long n, p, cols, total;   // N, P, columns per member (N / R), batch * cols
     long long in_rs, out_rs;       // elements between rows
-    long long bstride;             // elements between members of the caller's arrays (complex values for C2R_HALVED and C2C_IL*)
+    long long bstride;             // elements between members of the caller's arrays (complex values for C2R_HALVED, C2C_IL* and
+                                   // R2C_DIRECT_IL)
     int role, r, qb, lo_bits;
     int nstages, rad[ODD_MAX_STAGES];
     int cw;                        // tile kernel: columns per CTA
@@ -1267,7 +1328,7 @@ struct OddCol {
     T* out_re;
     T* out_im;
     cx<T>* out_y;                      // C2R_HALVED: the caller's real array as pairs (bstride counts pairs); C2C_IL*: its
-                                       // interleaved array
+                                       // interleaved array; R2C_DIRECT_IL: its interleaved bins
     int kmax;                          // R2C_DIRECT: the last row whose output index c + k out_rs is a stored bin (<= N/2)
     unsigned long long e0, de;
     __device__ __forceinline__ OddCol(const OddParams<T>& p, long long g) {
@@ -1279,8 +1340,9 @@ struct OddCol {
         out_c = p.ws_out + m * p.n + c;
         out_re = p.out_re + m * p.bstride + c;
         out_im = p.out_im + m * p.bstride + c;
-        if constexpr (MODE == CHIRP_C2R_HALVED || chirp_il<MODE>()) out_y = reinterpret_cast<cx<T>*>(p.out_re) + m * p.bstride + c;
-        if constexpr (MODE == CHIRP_R2C_DIRECT) kmax = (int)((p.n / 2 - c) / p.out_rs);      // c < N / 3 on the last pass
+        if constexpr (MODE == CHIRP_C2R_HALVED || chirp_il<MODE>() || MODE == CHIRP_R2C_DIRECT_IL)
+            out_y = reinterpret_cast<cx<T>*>(p.out_re) + m * p.bstride + c;
+        if constexpr (chirp_planar<MODE>() == CHIRP_R2C_DIRECT) kmax = (int)((p.n / 2 - c) / p.out_rs);      // c < N / 3 on the last pass
     }
     // row r, times W_N^(e0 + r de)
     __device__ __forceinline__ cx<T> load(const OddParams<T>& p, int r) const {
@@ -1298,6 +1360,9 @@ struct OddCol {
         } else if constexpr (MODE == CHIRP_C2R_DIRECT) {
             out_re[k * p.out_rs] = v.y * p.scale;                               // the real part of the inverse, / N
         } else if constexpr (chirp_il<MODE>()) {
+            out_y[k * p.out_rs] = il_store<T, MODE>(v, p.scale);
+        } else if constexpr (MODE == CHIRP_R2C_DIRECT_IL) {
+            if (k > kmax) return;                                               // bins 0 .. floor(N/2) only, as R2C_DIRECT
             out_y[k * p.out_rs] = il_store<T, MODE>(v, p.scale);
         } else {
             // R2C_DIRECT: the caller holds bins 0 .. floor(N/2) only
@@ -1434,7 +1499,8 @@ bool launch_odd_kernel(const OddParams<T>& q, int r, size_t smem, unsigned grid,
 // SMOOTH-PRE: ws[m N + n_o P + n_2] = (re, im)[m bstride + n_o + Q n_2].  A block transposes a tile of tq values of n_o by
 // tp values of n_2 through shared memory: it reads runs of tq adjacent elements and writes runs of tp adjacent complex values
 // (the plan picks tq * tp <= 1024 with the runs as long as Q and P allow).  The real modes load element n of z instead, the
-// interleaved ones complex value n of in_re (bstride is the input's member stride in T either way).
+// interleaved ones complex value n of in_re (bstride is the input's member stride in T either way; the c2r modes with an
+// interleaved spectrum read its bins from in_re).
 constexpr int SMOOTH_TILE = 1024;
 template <typename T>
 struct SmoothParams {
@@ -1458,10 +1524,13 @@ __device__ __forceinline__ cx<T> two_level_root(const cx<T>* hi, const cx<T>* lo
 // SMOOTH-PRE's element n of a real mode's z, from the member's input re / im
 template <typename T, int MODE>
 __device__ __forceinline__ cx<T> smooth_real_in(const SmoothParams<T>& p, const T* re, const T* im, long long n) {
-    if constexpr (MODE == CHIRP_R2C_HALVED) return reinterpret_cast<const cx<T>*>(re)[n];     // (x[2n], x[2n+1]), pair-aligned
-    else if constexpr (MODE == CHIRP_R2C_DIRECT) return make_cx<T>(re[n], T(0));
-    else if constexpr (MODE == CHIRP_C2R_HALVED) return c2r_halved_in<T>(re, im, p.n, n, two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, n));
-    else return c2r_direct_in<T>(re, im, p.n, n);
+    constexpr int PM = chirp_planar<MODE>();
+    constexpr bool SIL = chirp_spec_il<MODE>();
+    if constexpr (PM == CHIRP_R2C_HALVED) return reinterpret_cast<const cx<T>*>(re)[n];     // (x[2n], x[2n+1]), pair-aligned
+    else if constexpr (PM == CHIRP_R2C_DIRECT) return make_cx<T>(re[n], T(0));
+    else if constexpr (PM == CHIRP_C2R_HALVED)
+        return c2r_halved_in<T>(spec_at<T, SIL>(re, im, 0), p.n, n, two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, n));
+    else return c2r_direct_in<T>(spec_at<T, SIL>(re, im, 0), p.n, n);
 }
 
 template <typename T, int MODE = CHIRP_C2C>
@@ -1491,29 +1560,29 @@ __global__ void __launch_bounds__(256) smooth_pre_kernel(const __grid_constant__
 
 // SMOOTH-POST-R2C, the halved r2c's untangle in place: the last ODD pass stored Z = DFT_L(z) in bins 0 .. L-1 of the caller's
 // arrays; the thread of pair (k, L - k), k <= L/2, replaces Z[k] and Z[L - k] with X[k] and X[L - k] (k = 0: X[0] and X[L];
-// L even: k = L/2 is the self pair).  A member-major grid of 256-thread blocks.
+// L even: k = L/2 is the self pair).  A member-major grid of 256-thread blocks.  SIL: the bins are interleaved at re
+// (SMOOTH-POST-R2C-IL).
 template <typename T>
 struct SmoothPostParams {
     T* re;
     T* im;
     const cx<T>* wn_hi;            // W_(2L) two-level, as SmoothParams
     const cx<T>* wn_lo;
-    long long l, bstride;
+    long long l, bstride;          // bstride: elements of each array between members (interleaved: complex values)
     int lo_bits;
     unsigned blocks_per_member;
 };
-template <typename T>
+template <typename T, bool SIL = false>
 __global__ void __launch_bounds__(256) smooth_post_r2c_kernel(const __grid_constant__ SmoothPostParams<T> p) {
     const unsigned mb = blockIdx.x / p.blocks_per_member;
     const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * 256 + threadIdx.x;
     if (2 * k > p.l) return;
-    T* re = p.re + (long long)mb * p.bstride;
-    T* im = p.im + (long long)mb * p.bstride;
+    const SpecBins<T, SIL> y = spec_at<T, SIL>(p.re, p.im, (long long)mb * p.bstride);
     const long long m = p.l - k, mm = k ? m : 0;
     cx<T> xk, xm;
-    r2c_untangle<T>(make_cx<T>(re[k], im[k]), make_cx<T>(re[mm], im[mm]), two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, k), xk, xm);
-    re[k] = xk.x; im[k] = xk.y;
-    if (m != k) { re[m] = xm.x; im[m] = xm.y; }
+    r2c_untangle<T>(y.get(k), y.get(mm), two_level_root<T>(p.wn_hi, p.wn_lo, p.lo_bits, k), xk, xm);
+    y.put(k, xk.x, xk.y);
+    if (m != k) y.put(m, xm.x, xm.y);
 }
 
 }  // namespace phast

@@ -90,6 +90,7 @@ const char* mode_name(int mode) {
         case MODE_BULK_IN: return "bulk";
         case MODE_ROW_BULK: return "row-bulk";
         case MODE_C2R_IN: return "c2r-in";
+        case MODE_C2R_IN_IL: return "c2r-in-il";
         default: return "plain";
     }
 }
@@ -162,6 +163,7 @@ const std::vector<KernelEntry<T>>& registry() {
         add_row_kernels<T>(v);                       // whole transform in one CTA (rows contiguous in and out)
         add_strided_kernels<T, KIND_COL>(v);         // first / middle passes
         add_strided_kernels<T, KIND_TRANS>(v);       // last pass
+        add_c2r_il_kernels<T>(v);                    // the interleaved-spectrum twins of the first passes' c2r builds
         return v;
     }();
     return reg;
@@ -277,6 +279,8 @@ struct PassDesc {
     const KernelEntry<T>* kt = nullptr;   // 2-pass plans of lone transforms: the pass with an asynchronous (TMA) tile input
     const KernelEntry<T>* kc = nullptr;   // first pass only: `k` with the c2r pre-processing folded into its loads (MODE_C2R_IN)
     const KernelEntry<T>* kcb = nullptr;  // first pass only: the same build of `kb` (batched c2r)
+    const KernelEntry<T>* kci = nullptr;  // kc and kcb reading interleaved bins (MODE_C2R_IN_IL): present wherever those are
+    const KernelEntry<T>* kcbi = nullptr;
     const KernelEntry<T>* kr = nullptr;   // one-CTA plans: `kb` with its tile moved in and out by cp.async.bulk (MODE_ROW_BULK)
     size_t tw_wc_off_t = (size_t)-1;      // W_L^(c*m) table for `kt`
     size_t tw_im_off = (size_t)-1;        // one-CTA kernels: the per-stage [i][m] stage-twiddle tables for `k` ...
@@ -615,13 +619,22 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
         if (!d.k) return fail(PHASTFT_ERR_INVALID_ARG, "no kernel for pass size 2^" + std::to_string(f[p]) + " kind " + kind_name(kind));
         if (kind == KIND_ROW) d.kr = find_row_bulk<T>(d.kb);
         if (p == 0 && kind == KIND_COL)         // the same tile with the c2r pre-processing in its loads, if compiled (c2r_dev uses it)
-            for (const auto& e : registry<T>())
-                if (e.mode == MODE_C2R_IN && !e.batch_only && e.kind == kind && e.R == d.k->R && e.C == d.k->C && e.NT == d.k->NT &&
-                    e.variant == d.k->variant && e.rl == d.k->rl) d.kc = &e;
+            for (const auto& e : registry<T>()) {
+                const bool same = e.kind == kind && e.R == d.k->R && e.C == d.k->C && e.NT == d.k->NT && e.variant == d.k->variant &&
+                                  e.rl == d.k->rl && !e.batch_only;
+                if (same && e.mode == MODE_C2R_IN) d.kc = &e;
+                if (same && e.mode == MODE_C2R_IN_IL) d.kci = &e;
+            }
         if (p == 0 && kind == KIND_COL && d.kb)  // ... and of the batch tile (batched c2r)
-            for (const auto& e : registry<T>())
-                if (e.mode == MODE_C2R_IN && e.kind == kind && e.R == d.kb->R && e.C == d.kb->C && e.NT == d.kb->NT &&
-                    e.variant == d.kb->variant && e.rl == d.kb->rl) d.kcb = &e;
+            for (const auto& e : registry<T>()) {
+                const bool same = e.kind == kind && e.R == d.kb->R && e.C == d.kb->C && e.NT == d.kb->NT && e.variant == d.kb->variant &&
+                                  e.rl == d.kb->rl;
+                if (same && e.mode == MODE_C2R_IN) d.kcb = &e;
+                if (same && e.mode == MODE_C2R_IN_IL) d.kcbi = &e;
+            }
+        // the interleaved c2r takes the planar one's path, so every c2r build has its interleaved twin (one tile list, reg_strided.cu)
+        if ((d.kc != nullptr) != (d.kci != nullptr) || (d.kcb != nullptr) != (d.kcbi != nullptr))
+            return fail(PHASTFT_ERR_INVALID_ARG, "unreachable: a c2r build of the first pass has no interleaved twin");
         if (p > 0) {
             d.has_tw = 1;
             d.log2Rprev = f[p - 1];
@@ -834,6 +847,10 @@ int32_t build_plan(size_t n, int device, Plan<T>** out) {
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kc->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kc->smem));
         if (pl->pass[p].kcb)
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kcb->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kcb->smem));
+        if (pl->pass[p].kci)
+            CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kci->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kci->smem));
+        if (pl->pass[p].kcbi)
+            CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kcbi->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kcbi->smem));
         if (pl->pass[p].kr)
             CUDA_TRY(cudaFuncSetAttribute(pl->pass[p].kr->fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pl->pass[p].kr->smem));
     }
@@ -990,7 +1007,7 @@ struct Io {
     long long in_bstride, out_bstride;
     int in_il, out_il;   // 0 planar, 1 interleaved, 2 interleaved with re/im swapped
     // c2r: in_re / in_im are the half-spectrum's N/2 + 1 bins and the first pass builds its input from them while loading
-    // (PassDesc::kc); pre_log2half = log2(N/2), 0 = off
+    // (PassDesc::kc; in_il = 1: the bins interleaved at in_re, PassDesc::kci); pre_log2half = log2(N/2), 0 = off
     Tw2 pre_tw2 = {nullptr, nullptr, 0};
     int pre_log2half = 0;
     const double2* pre_wc = nullptr;     // host: W_(2 R1)^i, i < 32 (PlanR2c::pre_wc)
@@ -1081,7 +1098,8 @@ int32_t prepare_pass_desc(const Plan<T>& pl, const PassDesc<T>& d, int p, const 
           reinterpret_cast<uintptr_t>(base.out_im)) & 15) == 0)
         k = d.kr;
     if (base.pre_log2half) {
-        const KernelEntry<T>* kc = many ? d.kcb : d.kc;
+        // interleaved bins (in_interleaved = 1): the MODE_C2R_IN_IL twin of the same tile
+        const KernelEntry<T>* kc = base.in_interleaved ? (many ? d.kcbi : d.kci) : many ? d.kcb : d.kc;
         if (p != 0 || use_kt || !kc) return fail(PHASTFT_ERR_INVALID_ARG, "c2r pre-processing on load: first pass with a MODE_C2R_IN kernel only");
         k = kc;
     }
@@ -1985,22 +2003,30 @@ Tw2 r2c_tw2(const PlanR2c<T>* pl) {
 
 // The elementwise r2c untangle / c2r pre-processing of `members` batch members, `per` threads each: a member-major grid of
 // 256-thread blocks, so a batch is not capped by gridDim.y; a batch of more than 2^31 - 1 blocks takes several launches.
-// Launch record: R = N/2, C = the members of that launch.
+// Launch record: R = N/2, C = the members of that launch.  `il`: the spectrum's bins are interleaved (the untangle's re, the
+// pre-processing's in_re; im / in_im unused, strides in complex values): R2C-UNTANGLE-IL / C2R-PRE-IL.
 template <typename T>
-int32_t launch_real(bool untangle, const RealParams<T>& rp, size_t per, size_t members, cudaStream_t stream) {
+int32_t launch_real(bool untangle, const RealParams<T>& rp, size_t per, size_t members, cudaStream_t stream, bool il = false) {
     const size_t bpm = (per + 255) / 256;
     const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t out_w = il && untangle ? 2 : 1, in_w = il && !untangle ? 2 : 1;   // T per bin of the interleaved side
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
         RealParams<T> q = rp;
-        q.re += done * rp.bstride; q.im += done * rp.bstride;
-        if (q.in_re) { q.in_re += done * rp.in_bstride; q.in_im += done * rp.in_bstride; }
+        q.re += out_w * done * rp.bstride;
+        if (q.im) q.im += done * rp.bstride;
+        if (q.in_re) {
+            q.in_re += in_w * done * rp.in_bstride;
+            if (q.in_im) q.in_im += done * rp.in_bstride;
+        }
         q.blocks_per_member = (unsigned)bpm;
         const dim3 grid((unsigned)(nb * bpm));
-        if (untangle) r2c_untangle_kernel<T><<<grid, 256, 0, stream>>>(q);
+        if (il) launch_real_il<T>(untangle, q, grid.x, stream);
+        else if (untangle) r2c_untangle_kernel<T><<<grid, 256, 0, stream>>>(q);
         else c2r_preprocess_kernel<T><<<grid, 256, 0, stream>>>(q);
         CUDA_TRY(cudaGetLastError());
-        note_launch({untangle ? "R2C-UNTANGLE" : "C2R-PRE", 1 << rp.log2half, 0, (int)nb, 256, 0, "plain", false});
+        note_launch({untangle ? (il ? "R2C-UNTANGLE-IL" : "R2C-UNTANGLE") : il ? "C2R-PRE-IL" : "C2R-PRE", 1 << rp.log2half, 0, (int)nb, 256, 0,
+                     "plain", false});
     }
     return PHASTFT_OK;
 }
@@ -2274,6 +2300,69 @@ int32_t r2c_reserve(const PlanR2c<T>* pl, size_t batch) {
     DeviceGuard g(pl->device);
     std::lock_guard<std::mutex> lock(pl->mu);
     return grow_r2c_scratch(pl, batch * (pl->n / 2));
+}
+
+// Interleaved spectra (phastft_{r2c,c2r}_interleaved_any_* on a power of two): member b's N/2 + 1 bins are Complex<T> values at
+// complex element b * stride of d_spec.  The calls run the launches of r2c_batch_dev / c2r_batch_dev (c2r_dev for one member,
+// with the plan's scratch) with the interleaved layout at the spectrum's end: the last pass stores Z as Complex<T>
+// (out_interleaved = 1) and R2C-UNTANGLE-IL untangles it in place; c2r reads the bins in the MODE_C2R_IN_IL first pass or in
+// C2R-PRE-IL.  Same arithmetic, so the planar call's results bit for bit.  The caller checked the arguments.
+template <typename T>
+int32_t r2c_il_dev(const PlanR2c<T>* pl, const T* d_in, size_t in_stride, T* d_spec, size_t spec_stride, size_t batch, cudaStream_t stream) {
+    DeviceGuard g(pl->device);
+    const size_t half = pl->n / 2;
+    Io<T> io;
+    io.in_re = d_in; io.in_im = nullptr; io.in_il = 1; io.in_bstride = (long long)(batch > 1 ? in_stride / 2 : half);
+    io.out_re = d_spec; io.out_im = nullptr; io.out_il = 1; io.out_bstride = (long long)(batch > 1 ? spec_stride : half);
+    if (int32_t st = run_c2c(*pl->inner, io, batch, T(1), stream)) return st;
+    RealParams<T> rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.re = d_spec; rp.im = nullptr; rp.bstride = (long long)(batch > 1 ? spec_stride : 0); rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
+    return launch_real(true, rp, half / 2 + 1, batch, stream, true);
+}
+
+template <typename T>
+int32_t c2r_il_dev(const PlanR2c<T>* pl, const T* d_spec, size_t spec_stride, T* d_out, size_t out_stride, size_t batch, cudaStream_t stream) {
+    DeviceGuard g(pl->device);
+    const size_t half = pl->n / 2;
+    Io<T> io;
+    io.out_re = d_out; io.out_im = nullptr; io.out_il = 2; io.out_bstride = (long long)(batch > 1 ? out_stride / 2 : half);
+    if (c2r_fuses(pl, batch, nullptr)) {
+        io.in_re = d_spec; io.in_im = nullptr; io.in_il = 1; io.in_bstride = (long long)(batch > 1 ? spec_stride : half);
+        io.pre_tw2 = r2c_tw2(pl); io.pre_log2half = ilog2(half); io.pre_wc = pl->pre_wc;
+        if (batch > 1) io.pre_wc_b = pl->pre_wc_b;
+        return run_c2c(*pl->inner, io, batch, T(1) / (T)half, stream);
+    }
+    // the separate sweep into the plan-owned scratch, under c2r_batch_dev's protocol (c2r_dev's for one member)
+    std::lock_guard<std::mutex> lock(pl->mu);
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    CUDA_TRY(cudaStreamIsCapturing(stream, &cap));
+    const bool capturing = cap != cudaStreamCaptureStatusNone;
+    if (pl->scr_elems < batch * half) {
+        if (capturing)
+            return fail(PHASTFT_ERR_INVALID_ARG, "the plan's c2r scratch is too small for this batch and the stream is being captured: "
+                                                 "call phastft_plan_r2c_any_*_reserve(batch) before capturing");
+        if (int32_t st = grow_r2c_scratch(pl, batch * half)) return st;
+    }
+    T* sre = pl->d_scr_re;
+    T* sim = pl->d_scr_im;
+    if (!capturing && pl->scr_used && pl->scr_last_stream != stream) CUDA_TRY(cudaStreamWaitEvent(stream, pl->scr_free, 0));
+    CUDA_TRY(scribble(pl->inner->scribble_on, sre, batch * half * sizeof(T), stream));
+    CUDA_TRY(scribble(pl->inner->scribble_on, sim, batch * half * sizeof(T), stream));
+    RealParams<T> rp;
+    memset(&rp, 0, sizeof(rp));
+    rp.re = sre; rp.im = sim; rp.bstride = (long long)(batch > 1 ? half : 0);
+    rp.in_re = d_spec; rp.in_im = nullptr; rp.in_bstride = (long long)(batch > 1 ? spec_stride : 0);
+    rp.log2half = ilog2(half); rp.tw2 = r2c_tw2(pl);
+    if (int32_t st = launch_real(false, rp, half, batch, stream, true)) return st;
+    io.in_re = sim; io.in_im = sre; io.in_il = 0; io.in_bstride = (long long)half;
+    int32_t st = run_c2c(*pl->inner, io, batch, T(1) / (T)half, stream);
+    if (st == PHASTFT_OK && !capturing) {
+        CUDA_TRY(cudaEventRecord(pl->scr_free, stream));
+        pl->scr_last_stream = stream;
+        pl->scr_used = true;
+    }
+    return st;
 }
 
 template <typename T>
@@ -2610,11 +2699,13 @@ int32_t build_mixed(Mixed<T>& mx, size_t n, const MixedSplit& split, int device)
                                   ODD_MAX_ROWS * 128));
     CUDA_TRY(mixed_real_init<T>());
     CUDA_TRY(any_il_init<T>());
+    CUDA_TRY(real_il_init<T>());
     return mx.w.init(n);                               // room for one member; batched calls grow it
 }
 
 // One ODD pass over `batch` members, MODE the last pass's store (C2C for pass A).  Launch record: R = rows, C = the columns a
-// CTA covers; the kind carries -C2R / -R2C for the real stores, -IL for the interleaved ones.
+// CTA covers; the kind carries -C2R / -R2C for the real stores, -IL for the interleaved ones (ODD-R2C-IL: the direct r2c's
+// interleaved bins).
 template <int MODE, typename T>
 int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cudaStream_t stream) {
     const OddPass<T>& ps = mx.pass[i];
@@ -2635,10 +2726,12 @@ int32_t launch_odd(const Mixed<T>& mx, int i, OddParams<T> q, size_t batch, cuda
     const size_t smem = ps.cw ? (size_t)ps.r * ps.cw * sizeof(cx<T>) : 0;
     const bool ok = MODE == CHIRP_C2C ? launch_odd_kernel<T, CHIRP_C2C>(q, ps.r, smem, (unsigned)blocks, stream)
                     : chirp_il<MODE>() ? launch_odd_il<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream)
+                    : MODE == CHIRP_R2C_DIRECT_IL ? launch_odd_r2c_il<T>(q, ps.r, smem, (unsigned)blocks, stream)
                                        : launch_odd_real<T>(MODE, q, ps.r, smem, (unsigned)blocks, stream);
     if (!ok) return fail(PHASTFT_ERR_INVALID_ARG, "no register kernel of " + std::to_string(ps.r) + " rows");
     CUDA_TRY(cudaGetLastError());
     const char* name = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT ? "ODD-C2R" : MODE == CHIRP_R2C_DIRECT ? "ODD-R2C"
+                       : MODE == CHIRP_R2C_DIRECT_IL                        ? "ODD-R2C-IL"
                        : chirp_il<MODE>()                                   ? "ODD-IL"
                                                                             : "ODD";
     note_launch({name, ps.r, 0, cover, ODD_NT, 0, ps.cw ? "tile" : "reg", false});
@@ -2679,12 +2772,19 @@ int32_t build_two_level(TwoLevelRoots<T>& t, size_t n, size_t count) {
 // interleaved modes: in_re and out_re, swapped by the mode); in_bstride counts T, out_bstride what the last pass stores (T, or
 // complex values for C2R_HALVED and the interleaved modes); scale is 1, 1/N or 1/L.  `wn` is the real plan's W_(2L) for the
 // halved modes.  The halved r2c ends with SMOOTH-POST-R2C on the bins.  The workspace follows AnyWorkspace's protocol (`reserve_fn` names the call that grows it).
+// The real modes with an interleaved spectrum (CHIRP_*_IL, spectrum strides in complex values) run their mode at the spectrum's
+// end only: r2c loads with the planar SMOOTH-PRE-R2C and stores ODD-IL + SMOOTH-POST-R2C-IL (halved) or ODD-R2C-IL (direct);
+// c2r loads with SMOOTH-PRE-C2R-IL and stores with the planar ODD-C2R.
 template <int MODE, typename T>
 int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_bstride, T* out_re, T* out_im, size_t out_bstride,
                   T scale, size_t batch, cudaStream_t stream, const char* reserve_fn, const TwoLevelRoots<T>* wn = nullptr) {
-    constexpr bool r2c = MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT, c2r = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT;
+    constexpr int PM = chirp_planar<MODE>();
+    constexpr bool sil = chirp_spec_il<MODE>();
+    constexpr bool r2c = PM == CHIRP_R2C_HALVED || PM == CHIRP_R2C_DIRECT, c2r = PM == CHIRP_C2R_HALVED || PM == CHIRP_C2R_DIRECT;
     constexpr bool il = chirp_il<MODE>();
-    constexpr int LAST = MODE == CHIRP_R2C_HALVED ? CHIRP_C2C : MODE;   // the halved r2c stores Z, then untangles it in place
+    constexpr int PRE = r2c ? PM : MODE;                                // SMOOTH-PRE's mode
+    // the halved r2c stores Z, then untangles it in place
+    constexpr int LAST = MODE == CHIRP_R2C_HALVED ? CHIRP_C2C : MODE == CHIRP_R2C_HALVED_IL ? CHIRP_C2C_IL : c2r ? PM : MODE;
     DeviceGuard g(mx.device);
     const size_t P = mx.split.p, Q = (size_t)mx.split.qa * mx.split.qb;
     std::lock_guard<std::mutex> lock(mx.w.mu);
@@ -2711,10 +2811,11 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
         if (s2.in_im) s2.in_im += done * in_bstride;
         if constexpr (MODE == CHIRP_C2C) smooth_pre_kernel<T><<<(unsigned)(nb * sp.tiles_per_member), 256, 0, stream>>>(s2);
         else if constexpr (il) launch_smooth_pre_il<T>(MODE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
-        else launch_smooth_pre_real<T>(MODE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
+        else if constexpr (chirp_spec_il<PRE>()) launch_smooth_pre_real_il<T>(PRE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
+        else launch_smooth_pre_real<T>(PRE, s2, (unsigned)(nb * sp.tiles_per_member), stream);
         CUDA_TRY(cudaGetLastError());
-        note_launch({r2c ? "SMOOTH-PRE-R2C" : c2r ? "SMOOTH-PRE-C2R" : il ? "SMOOTH-PRE-IL" : "SMOOTH-PRE", (int)P, 0, (int)(nb * Q), 256, 0,
-                     "plain", false});
+        note_launch({r2c ? "SMOOTH-PRE-R2C" : c2r ? (sil ? "SMOOTH-PRE-C2R-IL" : "SMOOTH-PRE-C2R") : il ? "SMOOTH-PRE-IL" : "SMOOTH-PRE",
+                     (int)P, 0, (int)(nb * Q), 256, 0, "plain", false});
     }
     if (P > 1) {
         Io<T> io;
@@ -2732,7 +2833,7 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
     for (int i = 0; i < mx.npasses; ++i)
         if (int32_t st = i + 1 < mx.npasses ? launch_odd<CHIRP_C2C>(mx, i, q, batch, stream) : launch_odd<LAST>(mx, i, q, batch, stream))
             return st;
-    if constexpr (MODE == CHIRP_R2C_HALVED) {
+    if constexpr (PM == CHIRP_R2C_HALVED) {
         // Launch record: R = L, C = the members of that launch
         SmoothPostParams<T> pp;
         pp.re = out_re; pp.im = out_im; pp.wn_hi = wn->hi; pp.wn_lo = wn->lo; pp.lo_bits = wn->lo_bits;
@@ -2743,10 +2844,12 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
         for (size_t done = 0; done < batch; done += max_members) {
             const size_t nb = std::min(batch - done, max_members);
             SmoothPostParams<T> p2 = pp;
-            p2.re += done * out_bstride; p2.im += done * out_bstride;
-            launch_smooth_post_r2c<T>(p2, (unsigned)(nb * bpm), stream);
+            p2.re += (sil ? 2 : 1) * done * out_bstride;
+            if (p2.im) p2.im += done * out_bstride;
+            if constexpr (sil) launch_smooth_post_r2c_il<T>(p2, (unsigned)(nb * bpm), stream);
+            else launch_smooth_post_r2c<T>(p2, (unsigned)(nb * bpm), stream);
             CUDA_TRY(cudaGetLastError());
-            note_launch({"SMOOTH-POST-R2C", (int)mx.n, 0, (int)nb, 256, 0, "plain", false});
+            note_launch({sil ? "SMOOTH-POST-R2C-IL" : "SMOOTH-POST-R2C", (int)mx.n, 0, (int)nb, 256, 0, "plain", false});
         }
     }
     return mx.w.release(stream, capturing);
@@ -2916,13 +3019,17 @@ enum ChirpKind { CHIRP_PRE, CHIRP_MUL, CHIRP_POST };
 
 // One CHIRP-* kernel over `members` batch members, `per` threads each: a member-major grid of 256-thread blocks (as launch_real),
 // several launches when it would exceed 2^31 - 1 blocks.  Launch record: R = M, C = the members of that launch; the kind carries
-// -R2C / -C2R for the real modes' CHIRP-PRE and CHIRP-POST, -IL for the interleaved ones.
+// -R2C / -C2R for the real modes' CHIRP-PRE and CHIRP-POST, -IL for the interleaved ones.  The real modes with an interleaved
+// spectrum run it at the spectrum's end only (CHIRP-POST-R2C-IL, CHIRP-PRE-C2R-IL) and the planar mode's kernel at the other.
 template <int MODE, typename T>
 int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_t members, cudaStream_t stream) {
     const size_t bpm = (per + 255) / 256;
     const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
-    constexpr bool r2c = MODE == CHIRP_R2C_HALVED || MODE == CHIRP_R2C_DIRECT, c2r = MODE == CHIRP_C2R_HALVED || MODE == CHIRP_C2R_DIRECT;
+    constexpr int PM = chirp_planar<MODE>();
+    constexpr bool r2c = PM == CHIRP_R2C_HALVED || PM == CHIRP_R2C_DIRECT, c2r = PM == CHIRP_C2R_HALVED || PM == CHIRP_C2R_DIRECT;
     constexpr bool il = chirp_il<MODE>();
+    constexpr int PRE = r2c ? PM : MODE, POST = c2r ? PM : MODE;
+    const bool sil = kind == CHIRP_PRE ? chirp_spec_il<PRE>() : chirp_spec_il<POST>();
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
         ChirpParams<T> q = cp;
@@ -2940,12 +3047,17 @@ int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_
         const dim3 grid((unsigned)(nb * bpm));
         if (kind == CHIRP_MUL) chirp_mul_kernel<T><<<grid, 256, 0, stream>>>(q);
         else if constexpr (il) launch_chirp_il<T>(MODE, kind == CHIRP_POST, q, grid.x, stream);
-        else if (kind == CHIRP_PRE) chirp_pre_kernel<T, MODE><<<grid, 256, 0, stream>>>(q);
-        else chirp_post_kernel<T, MODE><<<grid, 256, 0, stream>>>(q);
+        else if (kind == CHIRP_PRE) {
+            if constexpr (chirp_spec_il<PRE>()) launch_chirp_real_il<T>(PRE, q, grid.x, stream);
+            else chirp_pre_kernel<T, PRE><<<grid, 256, 0, stream>>>(q);
+        } else {
+            if constexpr (chirp_spec_il<POST>()) launch_chirp_real_il<T>(POST, q, grid.x, stream);
+            else chirp_post_kernel<T, POST><<<grid, 256, 0, stream>>>(q);
+        }
         CUDA_TRY(cudaGetLastError());
         const char* name = kind == CHIRP_MUL ? "CHIRP-MUL"
-                           : kind == CHIRP_PRE ? (r2c ? "CHIRP-PRE-R2C" : c2r ? "CHIRP-PRE-C2R" : il ? "CHIRP-PRE-IL" : "CHIRP-PRE")
-                                               : (r2c ? "CHIRP-POST-R2C" : c2r ? "CHIRP-POST-C2R" : il ? "CHIRP-POST-IL" : "CHIRP-POST");
+                           : kind == CHIRP_PRE ? (r2c ? "CHIRP-PRE-R2C" : c2r ? (sil ? "CHIRP-PRE-C2R-IL" : "CHIRP-PRE-C2R") : il ? "CHIRP-PRE-IL" : "CHIRP-PRE")
+                                               : (r2c ? (sil ? "CHIRP-POST-R2C-IL" : "CHIRP-POST-R2C") : c2r ? "CHIRP-POST-C2R" : il ? "CHIRP-POST-IL" : "CHIRP-POST");
         note_launch({name, 1 << cp.log2m, 0, (int)nb, 256, 0, "plain", false});
     }
     return PHASTFT_OK;
@@ -3120,10 +3232,13 @@ struct PlanR2cAny {
     mutable T* stage_real = nullptr;   // host-API staging: N reals, floor(N/2) + 1 bins
     mutable T* stage_re = nullptr;
     mutable T* stage_im = nullptr;
+    mutable T* stage_il_real = nullptr;   // the interleaved host calls' staging (N reals, floor(N/2) + 1 complex bins), allocated
+    mutable T* stage_il_spec = nullptr;   // by the first such call
     std::string description;
     ~PlanR2cAny() {
         DeviceGuard g(device);
-        for (void* p : {(void*)wn, (void*)wn2.blob, (void*)stage_real, (void*)stage_re, (void*)stage_im})
+        for (void* p : {(void*)wn, (void*)wn2.blob, (void*)stage_real, (void*)stage_re, (void*)stage_im, (void*)stage_il_real,
+                        (void*)stage_il_spec})
             if (p) cudaFree(p);
         delete pow2;
     }
@@ -3268,6 +3383,74 @@ int32_t c2r_any_dev(const PlanR2cAny<T>* pl, const T* d_ire, const T* d_iim, siz
                       : bluestein_run<CHIRP_C2R_DIRECT>(pl->bs, cp, batch, stream, res);
 }
 
+// The same transforms with the spectrum as interleaved Complex<T> bins: member b's floor(N/2) + 1 bins start at complex element
+// b * spec_stride of d_spec (>= floor(N/2) + 1), aligned to 2 * sizeof(T).  The real side keeps the planar call's rules.  Every
+// path runs the planar call's launches with the spectrum's end kernels in their interleaved modes, so the results are the
+// planar call's bit for bit.
+template <typename T>
+int32_t check_spec_il(const PlanR2cAny<T>* pl, const T* d_real, const T* d_spec, size_t real_stride, size_t spec_stride, bool r2c) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (!d_real) return fail(PHASTFT_ERR_INVALID_ARG, r2c ? "d_input == NULL" : "d_output == NULL");
+    if (!d_spec) return fail(PHASTFT_ERR_INVALID_ARG, r2c ? "d_out == NULL" : "d_in == NULL");
+    const size_t n = pl->n, bins = n / 2 + 1;
+    const char* rs = r2c ? "in_stride" : "out_stride";
+    const char* ss = r2c ? "out_stride_complex" : "in_stride_complex";
+    if (real_stride < n) return fail(PHASTFT_ERR_INVALID_ARG, std::string(rs) + " must be >= N = " + std::to_string(n) + " (got " + std::to_string(real_stride) + ")");
+    if (spec_stride < bins)
+        return fail(PHASTFT_ERR_INVALID_ARG, std::string(ss) + " must be >= N/2 + 1 = " + std::to_string(bins) + " (got " + std::to_string(spec_stride) + ")");
+    if (n % 2 == 0) {   // the real side is read or written as pairs
+        if (real_stride % 2) return fail(PHASTFT_ERR_INVALID_ARG, std::string(rs) + " must be even for even N (the reals are accessed as pairs)");
+        if (int32_t st = check_pair_alignment(d_real, r2c ? "d_input" : "d_output")) return st;
+    }
+    return check_pair_alignment(d_spec, r2c ? "d_out" : "d_in");
+}
+
+template <typename T>
+int32_t r2c_il_any_dev(const PlanR2cAny<T>* pl, const T* d_in, size_t in_stride, T* d_out, size_t out_stride, size_t batch,
+                       cudaStream_t stream) {
+    if (int32_t st = check_spec_il(pl, d_in, d_out, in_stride, out_stride, true)) return st;
+    if (batch == 0) return PHASTFT_OK;
+    if (pl->pow2) return r2c_il_dev(pl->pow2, d_in, in_stride, d_out, out_stride, batch, stream);
+    const char* res = "phastft_plan_r2c_any_*_reserve";
+    if (pl->mx.inner)
+        return pl->halved ? mixed_run<CHIRP_R2C_HALVED_IL, T>(pl->mx, d_in, nullptr, in_stride, d_out, nullptr, out_stride, T(1), batch,
+                                                           stream, res, &pl->wn2)
+                          : mixed_run<CHIRP_R2C_DIRECT_IL, T>(pl->mx, d_in, nullptr, in_stride, d_out, nullptr, out_stride, T(1), batch,
+                                                           stream, res);
+    ChirpParams<T> cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.in_re = d_in; cp.out_re = d_out;
+    cp.bstride = (long long)in_stride; cp.out_bstride = 2 * (long long)out_stride;
+    cp.scale = T(1);
+    cp.wn = pl->wn;
+    return pl->halved ? bluestein_run<CHIRP_R2C_HALVED_IL>(pl->bs, cp, batch, stream, res)
+                      : bluestein_run<CHIRP_R2C_DIRECT_IL>(pl->bs, cp, batch, stream, res);
+}
+
+template <typename T>
+int32_t c2r_il_any_dev(const PlanR2cAny<T>* pl, const T* d_in, size_t in_stride, T* d_out, size_t out_stride, size_t batch,
+                       cudaStream_t stream) {
+    if (int32_t st = check_spec_il(pl, d_out, d_in, out_stride, in_stride, false)) return st;
+    if (batch == 0) return PHASTFT_OK;
+    if (pl->pow2) return c2r_il_dev(pl->pow2, d_in, in_stride, d_out, out_stride, batch, stream);
+    const char* res = "phastft_plan_r2c_any_*_reserve";
+    if (pl->mx.inner) {
+        const T scale = T(1) / (T)pl->mx.n;
+        return pl->halved ? mixed_run<CHIRP_C2R_HALVED_IL, T>(pl->mx, d_in, nullptr, 2 * in_stride, d_out, nullptr, out_stride / 2, scale,
+                                                           batch, stream, res, &pl->wn2)
+                          : mixed_run<CHIRP_C2R_DIRECT_IL, T>(pl->mx, d_in, nullptr, 2 * in_stride, d_out, nullptr, out_stride, scale,
+                                                           batch, stream, res);
+    }
+    ChirpParams<T> cp;
+    memset(&cp, 0, sizeof(cp));
+    cp.in_re = d_in; cp.out_re = d_out;
+    cp.bstride = 2 * (long long)in_stride; cp.out_bstride = (long long)out_stride;
+    cp.scale = T(1) / (T)pl->bs.l;
+    cp.wn = pl->wn;
+    return pl->halved ? bluestein_run<CHIRP_C2R_HALVED_IL>(pl->bs, cp, batch, stream, res)
+                      : bluestein_run<CHIRP_C2R_DIRECT_IL>(pl->bs, cp, batch, stream, res);
+}
+
 template <typename T>
 int32_t r2c_any_reserve(const PlanR2cAny<T>* pl, size_t batch) {
     if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
@@ -3308,6 +3491,59 @@ int32_t r2c_any_host(const PlanR2cAny<T>* pl, const T* in, size_t len_in, T* ore
     if (int32_t st = r2c_any_dev(pl, pl->stage_real, n, pl->stage_re, pl->stage_im, bins, 1, s)) return st;
     CUDA_TRY(cudaMemcpyAsync(ore, pl->stage_re, bins * sizeof(T), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(oim, pl->stage_im, bins * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
+// Caller holds host_mu: the interleaved host calls' staging, poisoned under PHASTFT_SCRIBBLE=1 like the planar one.  Allocated
+// under the lock the device call takes (the r2c plan's for a power of two, else the workspace's), released before that call.
+template <typename T>
+int32_t ensure_r2c_any_il_staging(const PlanR2cAny<T>* pl, cudaStream_t s) {
+    const size_t n = pl->n, bins = n / 2 + 1;
+    {
+        std::lock_guard<std::mutex> lock(pl->pow2 ? pl->pow2->mu : pl->workspace().mu);
+        if (!pl->stage_il_real) CUDA_TRY(cudaMalloc(&pl->stage_il_real, n * sizeof(T)));
+        if (!pl->stage_il_spec) CUDA_TRY(cudaMalloc(&pl->stage_il_spec, 2 * bins * sizeof(T)));
+    }
+    const bool on = pl->pow2 ? pl->pow2->inner->scribble_on : pl->workspace().scribble_on;
+    CUDA_TRY(scribble(on, pl->stage_il_real, n * sizeof(T), s));
+    CUDA_TRY(scribble(on, pl->stage_il_spec, 2 * bins * sizeof(T), s));
+    return PHASTFT_OK;
+}
+
+// interleaved host slices, synchronous: the planar host calls' length codes (spectrum lengths in complex values)
+template <typename T>
+int32_t r2c_il_any_host(const PlanR2cAny<T>* pl, const T* in, size_t len_in, T* out, size_t len_out) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const size_t n = pl->n, bins = n / 2 + 1;
+    if (len_in != n) return fail(PHASTFT_ERR_INPUT_LEN);
+    if (len_out != bins) return fail(PHASTFT_ERR_OUTPUT_RE_LEN);
+    if (!in || !out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->pow2 ? pl->pow2->inner->stream : pl->host_stream();
+    if (int32_t st = ensure_r2c_any_il_staging(pl, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(pl->stage_il_real, in, n * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = r2c_il_any_dev(pl, pl->stage_il_real, n, pl->stage_il_spec, bins, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(out, pl->stage_il_spec, 2 * bins * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
+template <typename T>
+int32_t c2r_il_any_host(const PlanR2cAny<T>* pl, const T* in, size_t len_in, T* out, size_t len_out) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const size_t n = pl->n, bins = n / 2 + 1;
+    if (len_out != n) return fail(PHASTFT_ERR_OUTPUT_LEN);
+    if (len_in != bins) return fail(PHASTFT_ERR_INPUT_RE_LEN);
+    if (!in || !out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->pow2 ? pl->pow2->inner->stream : pl->host_stream();
+    if (int32_t st = ensure_r2c_any_il_staging(pl, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(pl->stage_il_spec, in, 2 * bins * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = c2r_il_any_dev(pl, pl->stage_il_spec, bins, pl->stage_il_real, n, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(out, pl->stage_il_real, n * sizeof(T), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
     return PHASTFT_OK;
 }
@@ -3649,6 +3885,26 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                          size_t lore, T* oim, size_t loim) {                                            \
         launches_reset();                                                                                               \
         return r2c_any_host<T>(AS_CR2CANY(T, p), in, lin, ore, lore, oim, loim);                                        \
+    }                                                                                                                   \
+    int32_t phastft_r2c_interleaved_any_##SFX##_dev(const phastft_plan_r2c_any_##SFX* p, const T* in, size_t in_stride,  \
+                                                     T* out, size_t out_stride, size_t batch, void* s) {                \
+        launches_reset();                                                                                               \
+        return r2c_il_any_dev<T>(AS_CR2CANY(T, p), in, in_stride, out, out_stride, batch, (cudaStream_t)s);             \
+    }                                                                                                                   \
+    int32_t phastft_c2r_interleaved_any_##SFX##_dev(const phastft_plan_r2c_any_##SFX* p, const T* in, size_t in_stride,  \
+                                                     T* out, size_t out_stride, size_t batch, void* s) {                \
+        launches_reset();                                                                                               \
+        return c2r_il_any_dev<T>(AS_CR2CANY(T, p), in, in_stride, out, out_stride, batch, (cudaStream_t)s);             \
+    }                                                                                                                   \
+    int32_t phastft_r2c_interleaved_any_##SFX##_host(const phastft_plan_r2c_any_##SFX* p, const T* in, size_t lin,     \
+                                                      T* out, size_t lout) {                                            \
+        launches_reset();                                                                                               \
+        return r2c_il_any_host<T>(AS_CR2CANY(T, p), in, lin, out, lout);                                                \
+    }                                                                                                                   \
+    int32_t phastft_c2r_interleaved_any_##SFX##_host(const phastft_plan_r2c_any_##SFX* p, const T* in, size_t lin,     \
+                                                      T* out, size_t lout) {                                            \
+        launches_reset();                                                                                               \
+        return c2r_il_any_host<T>(AS_CR2CANY(T, p), in, lin, out, lout);                                                \
     }                                                                                                                   \
     int32_t phastft_c2r_any_##SFX##_host(const phastft_plan_r2c_any_##SFX* p, const T* ire, size_t lire, const T* iim,  \
                                          size_t liim, T* out, size_t lout) {                                            \

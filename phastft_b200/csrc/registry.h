@@ -3,7 +3,9 @@
 // The kernels are instantiated in several translation units so the library builds in parallel
 // (__graft_entry__.build()): reg_strided.cu (COL / TRANS passes, compiled once per precision and kind),
 // reg_row.cu (whole-transform-in-one-CTA kernels), reg_multi.cu (cluster and pipelined two-pass launches), mixed_real.cu (the
-// real modes of the mixed-radix kernels), any_interleaved.cu (the interleaved complex modes of the any-length end kernels).
+// real modes of the mixed-radix kernels), any_interleaved.cu (the interleaved complex modes of the any-length end kernels),
+// real_interleaved.cu (the interleaved-spectrum modes of the real transforms' end kernels) and reg_strided.cu again with
+// -DPHAST_C2R_IL (the MODE_C2R_IN_IL twins of the first-pass tiles, one unit per precision).
 // phastft_cuda.cu holds the planner, the launcher and the C ABI and only sees these descriptors.
 #pragma once
 #include <string>
@@ -17,7 +19,8 @@ template <typename T>
 struct KernelEntry {
     int kind, R, C, NT, first_radix, stages, variant;
     int mode = 0;          // MODE_PLAIN, MODE_TMA_IN / MODE_BULK_IN (asynchronous tile input), MODE_C2R_IN (c2r pre-processing on load)
-                           // or MODE_ROW_BULK (one-CTA batch kernel, tile in and out by cp.async.bulk)
+                           // or MODE_C2R_IN_IL (the same from interleaved bins), or MODE_ROW_BULK (one-CTA batch kernel, tile in and out
+                           // by cp.async.bulk)
     bool batch_only = false;   // MODE_C2R_IN builds of the batch first-pass tiles: never a lone transform's c2r build (PassDesc::kc),
                                // so adding one leaves every lone c2r on the path it had
     int rads[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // the stage radices (the planner builds the one-CTA kernels' [i][m] stage-twiddle tables from them)
@@ -89,27 +92,11 @@ KernelEntry<T> make_entry_async() {
     e.smem = PK::SMEM_BYTES;
     e.fn = reinterpret_cast<const void*>(&fft_pass_async_kernel<T, RL, C, NT, KIND, MODE, VARIANT, MINB>);
     e.rl = radix_string<RL>();
-    e.radices = e.rl + (MODE == MODE_TMA_IN ? ",tma" : MODE == MODE_BULK_IN ? ",bulk" : MODE == MODE_C2R_IN ? ",c2r" : ",bulk-io");
+    e.radices = e.rl + (MODE == MODE_TMA_IN ? ",tma" : MODE == MODE_BULK_IN ? ",bulk" : MODE == MODE_C2R_IN ? ",c2r"
+                        : MODE == MODE_C2R_IN_IL ? ",c2r-il" : ",bulk-io");
     for (int q = 0; q < RL::S && q < 8; ++q) e.rads[q] = RL::rad(q);
     if (ID) e.radices += ",v" + std::to_string(ID);
     return e;
-}
-
-// a default entry plus, for first-pass (COL) tiles, the same kernel with the c2r pre-processing folded into its loads
-template <typename T, int KIND, int C, int NT, int VARIANT, int MINB, int ID, int... Rs>
-void push_entry(std::vector<KernelEntry<T>>& v) {
-    v.push_back(make_entry_v<T, KIND, C, NT, VARIANT, MINB, ID, Rs...>());
-    if constexpr (KIND == KIND_COL) v.push_back(make_entry_async<T, KIND, C, NT, MODE_C2R_IN, VARIANT, MINB, ID, Rs...>());
-}
-// the same for a tile that is the first pass of batched calls only (PassDesc::kb): its c2r build serves batched c2r
-// (PassDesc::kcb) and is never looked up for a lone transform
-template <typename T, int KIND, int C, int NT, int VARIANT, int MINB, int ID, int... Rs>
-void push_entry_batch(std::vector<KernelEntry<T>>& v) {
-    v.push_back(make_entry_v<T, KIND, C, NT, VARIANT, MINB, ID, Rs...>());
-    if constexpr (KIND == KIND_COL) {
-        v.push_back(make_entry_async<T, KIND, C, NT, MODE_C2R_IN, VARIANT, MINB, ID, Rs...>());
-        v.back().batch_only = true;
-    }
 }
 
 template <typename T, int KIND, int C, int NT, int... Rs>
@@ -118,6 +105,7 @@ KernelEntry<T> make_entry() { return make_entry_v<T, KIND, C, NT, 0, 0, 0, Rs...
 // defined in the reg_*.cu translation units
 template <typename T> void add_row_kernels(std::vector<KernelEntry<T>>& v);
 template <typename T, int KIND> void add_strided_kernels(std::vector<KernelEntry<T>>& v);
+template <typename T> void add_c2r_il_kernels(std::vector<KernelEntry<T>>& v);   // reg_strided.cu with -DPHAST_C2R_IL
 template <typename T> const std::vector<PipeEntry<T>>& pipe_registry();
 template <typename T> const std::vector<ClusterEntry<T>>& cluster_registry();
 
@@ -134,5 +122,16 @@ template <typename T> cudaError_t any_il_init();
 template <typename T> bool launch_odd_il(int mode, const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
 template <typename T> void launch_smooth_pre_il(int mode, const SmoothParams<T>& p, unsigned grid, cudaStream_t stream);
 template <typename T> void launch_chirp_il(int mode, bool post, const ChirpParams<T>& p, unsigned grid, cudaStream_t stream);
+
+// defined in real_interleaved.cu: the interleaved-spectrum end kernels of the real transforms -- R2C-UNTANGLE-IL / C2R-PRE-IL
+// (`untangle`) of the power-of-two plan, CHIRP-POST of CHIRP_R2C_*_IL / CHIRP-PRE of CHIRP_C2R_*_IL (`mode`), SMOOTH-PRE of
+// CHIRP_C2R_*_IL, the last ODD pass of CHIRP_R2C_DIRECT_IL and SMOOTH-POST-R2C-IL; real_il_init sets the tile kernel's
+// shared-memory limit
+template <typename T> cudaError_t real_il_init();
+template <typename T> void launch_real_il(bool untangle, const RealParams<T>& p, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_chirp_real_il(int mode, const ChirpParams<T>& p, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_smooth_pre_real_il(int mode, const SmoothParams<T>& p, unsigned grid, cudaStream_t stream);
+template <typename T> bool launch_odd_r2c_il(const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
+template <typename T> void launch_smooth_post_r2c_il(const SmoothPostParams<T>& p, unsigned grid, cudaStream_t stream);
 
 }  // namespace phast

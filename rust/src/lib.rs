@@ -430,6 +430,50 @@ mod interleaved {
                           phastft_fft_interleaved_any_f64_host, phastft_fft_interleaved_any_f64_dev);
     impl_interleaved_any!(fft_32_interleaved_any_with_planner, fft_32_interleaved_any_device_batch, f32, PlannerAny32,
                           phastft_fft_interleaved_any_f32_host, phastft_fft_interleaved_any_f32_dev);
+
+    // Additive: real transforms of any length with the spectrum as interleaved bins
+    macro_rules! impl_real_interleaved_any {
+        ($r2c:ident, $c2r:ident, $r2c_dev:ident, $c2r_dev:ident, $t:ty, $planner:ident, $ffi_r2c_host:ident, $ffi_c2r_host:ident,
+         $ffi_r2c_dev:ident, $ffi_c2r_dev:ident) => {
+            /// N reals in, the floor(N/2) + 1 bins out as `Complex<T>`, forward unscaled; the planar call's results bit for bit.
+            /// Panics on a length mismatch.
+            pub fn $r2c(input: &[$t], output: &mut [Complex<$t>], planner: &$planner) {
+                check(unsafe { ffi::$ffi_r2c_host(planner.raw, input.as_ptr(), input.len(), output.as_mut_ptr() as *mut $t, output.len()) });
+            }
+            /// floor(N/2) + 1 `Complex<T>` bins in, N reals out, scaled so that c2r(r2c(x)) == x; the input is not written.
+            pub fn $c2r(input: &[Complex<$t>], output: &mut [$t], planner: &$planner) {
+                check(unsafe { ffi::$ffi_c2r_host(planner.raw, input.as_ptr() as *const $t, input.len(), output.as_mut_ptr(), output.len()) });
+            }
+            /// Device-resident: member b reads N reals at `d_input + b * in_stride` and writes its bins at complex element
+            /// `b * out_stride` of `d_out`, stream-ordered on `stream`.
+            ///
+            /// # Safety
+            /// Both pointers must be device pointers on the planner's device, valid for `batch` members at those strides
+            /// (`d_out` aligned to `Complex<T>`; for even N `d_input` aligned to 2 * size_of::<T>() and `in_stride` even), and
+            /// must not be used by other work on other streams until this call's work has completed.
+            pub unsafe fn $r2c_dev(d_input: *const $t, in_stride: usize, d_out: *mut Complex<$t>, out_stride: usize, planner: &$planner,
+                                   batch: usize, stream: *mut std::os::raw::c_void) {
+                check(ffi::$ffi_r2c_dev(planner.raw, d_input, in_stride, d_out as *mut $t, out_stride, batch, stream));
+            }
+            /// The mirror of the r2c batch: member b reads its bins at complex element `b * in_stride` of `d_in` and writes N
+            /// reals at `d_output + b * out_stride`.
+            ///
+            /// # Safety
+            /// As the r2c batch, with `d_in` aligned to `Complex<T>` and, for even N, `d_output` pair-aligned with an even stride.
+            pub unsafe fn $c2r_dev(d_in: *const Complex<$t>, in_stride: usize, d_output: *mut $t, out_stride: usize, planner: &$planner,
+                                   batch: usize, stream: *mut std::os::raw::c_void) {
+                check(ffi::$ffi_c2r_dev(planner.raw, d_in as *const $t, in_stride, d_output, out_stride, batch, stream));
+            }
+        };
+    }
+    impl_real_interleaved_any!(r2c_fft_f64_interleaved_any_with_planner, c2r_fft_f64_interleaved_any_with_planner,
+                               r2c_fft_f64_interleaved_any_device_batch, c2r_fft_f64_interleaved_any_device_batch, f64, PlannerR2cAny64,
+                               phastft_r2c_interleaved_any_f64_host, phastft_c2r_interleaved_any_f64_host,
+                               phastft_r2c_interleaved_any_f64_dev, phastft_c2r_interleaved_any_f64_dev);
+    impl_real_interleaved_any!(r2c_fft_f32_interleaved_any_with_planner, c2r_fft_f32_interleaved_any_with_planner,
+                               r2c_fft_f32_interleaved_any_device_batch, c2r_fft_f32_interleaved_any_device_batch, f32, PlannerR2cAny32,
+                               phastft_r2c_interleaved_any_f32_host, phastft_c2r_interleaved_any_f32_host,
+                               phastft_r2c_interleaved_any_f32_dev, phastft_c2r_interleaved_any_f32_dev);
 }
 #[cfg(feature = "complex-nums")]
 pub use interleaved::*;
