@@ -94,6 +94,14 @@ template <> struct Api<double> {
     static int32_t c2r_il_dev(const R2cAny* p, const double* in, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_interleaved_any_f64_dev(p, in, is, out, os, b, s); }
     static int32_t r2c_il_host(const R2cAny* p, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_r2c_interleaved_any_f64_host(p, in, li, out, lo); }
     static int32_t c2r_il_host(const R2cAny* p, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_c2r_interleaved_any_f64_host(p, in, li, out, lo); }
+    using Dct = phastft_plan_dct_f64;
+    static int32_t dct_create(std::size_t n, int dev, int algo, Dct** o) { return phastft_plan_dct_f64_create_with(n, dev, algo, o); }
+    static void dct_destroy(Dct* p) { phastft_plan_dct_f64_destroy(p); }
+    static std::size_t dct_size(const Dct* p) { return phastft_plan_dct_f64_size(p); }
+    static const char* dct_describe(const Dct* p) { return phastft_plan_dct_f64_describe(p); }
+    static int32_t dct_reserve(const Dct* p, std::size_t b) { return phastft_plan_dct_f64_reserve(p, b); }
+    static int32_t dct_dev(const Dct* p, int k, int nm, const double* in, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_dct_f64_dev(p, k, nm, in, is, out, os, b, s); }
+    static int32_t dct_host(const Dct* p, int k, int nm, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_dct_f64_host(p, k, nm, in, li, out, lo); }
 };
 template <> struct Api<float> {
     using Dit = phastft_plan_dit_f32; using R2c = phastft_plan_r2c_f32;
@@ -139,6 +147,14 @@ template <> struct Api<float> {
     static int32_t c2r_il_dev(const R2cAny* p, const float* in, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_c2r_interleaved_any_f32_dev(p, in, is, out, os, b, s); }
     static int32_t r2c_il_host(const R2cAny* p, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_r2c_interleaved_any_f32_host(p, in, li, out, lo); }
     static int32_t c2r_il_host(const R2cAny* p, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_c2r_interleaved_any_f32_host(p, in, li, out, lo); }
+    using Dct = phastft_plan_dct_f32;
+    static int32_t dct_create(std::size_t n, int dev, int algo, Dct** o) { return phastft_plan_dct_f32_create_with(n, dev, algo, o); }
+    static void dct_destroy(Dct* p) { phastft_plan_dct_f32_destroy(p); }
+    static std::size_t dct_size(const Dct* p) { return phastft_plan_dct_f32_size(p); }
+    static const char* dct_describe(const Dct* p) { return phastft_plan_dct_f32_describe(p); }
+    static int32_t dct_reserve(const Dct* p, std::size_t b) { return phastft_plan_dct_f32_reserve(p, b); }
+    static int32_t dct_dev(const Dct* p, int k, int nm, const float* in, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_dct_f32_dev(p, k, nm, in, is, out, os, b, s); }
+    static int32_t dct_host(const Dct* p, int k, int nm, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_dct_f32_host(p, k, nm, in, li, out, lo); }
 };
 
 /// planner.rs:34-114
@@ -291,6 +307,38 @@ class PlannerR2cAny {
   private:
     typename Api<T>::R2cAny* raw_ = nullptr;
 };
+
+/// additive: DCT / DST types 2 and 3 of any length with scipy.fft's definitions and norms, over an N-point real plan built with
+/// `algo`; R2rKind::Dct3 with the inverse norm is scipy's idct of type 2
+enum class R2rKind : int { Dct2 = PHASTFT_R2R_DCT2, Dct3 = PHASTFT_R2R_DCT3, Dst2 = PHASTFT_R2R_DST2, Dst3 = PHASTFT_R2R_DST3 };
+enum class R2rNorm : int { Backward = PHASTFT_NORM_BACKWARD, Ortho = PHASTFT_NORM_ORTHO, Forward = PHASTFT_NORM_FORWARD };
+template <typename T>
+class PlannerDct {
+  public:
+    explicit PlannerDct(std::size_t n, int device = 0, AnyAlgo algo = AnyAlgo::Auto) {
+        check(Api<T>::dct_create(n, device, static_cast<int>(algo), &raw_));
+    }
+    ~PlannerDct() { if (raw_) Api<T>::dct_destroy(raw_); }
+    PlannerDct(PlannerDct&& o) noexcept : raw_(o.raw_) { o.raw_ = nullptr; }
+    PlannerDct(const PlannerDct&) = delete;
+    PlannerDct& operator=(const PlannerDct&) = delete;
+    std::size_t n() const { return Api<T>::dct_size(raw_); }
+    /// "n=<N> <prec> dct | " followed by the inner real plan's description
+    std::string describe() const { return Api<T>::dct_describe(raw_); }
+    /// make every allocation a call of `batch` members would make now
+    void reserve(std::size_t batch) const { check(Api<T>::dct_reserve(raw_, batch)); }
+    /// N reals in, N out, on host vectors (`output` may be `input`)
+    void transform(R2rKind kind, R2rNorm norm, const std::vector<T>& input, std::vector<T>& output) const {
+        check(Api<T>::dct_host(raw_, static_cast<int>(kind), static_cast<int>(norm), input.data(), input.size(), output.data(), output.size()));
+    }
+    /// `batch` transforms on device pointers, member b at b * in_stride / b * out_stride (strides >= N, any offsets)
+    void transform_device(R2rKind kind, R2rNorm norm, const T* d_in, std::size_t in_stride, T* d_out, std::size_t out_stride,
+                          std::size_t batch, void* stream = nullptr) const {
+        check(Api<T>::dct_dev(raw_, static_cast<int>(kind), static_cast<int>(norm), d_in, in_stride, d_out, out_stride, batch, stream));
+    }
+  private:
+    typename Api<T>::Dct* raw_ = nullptr;
+};
 }  // namespace detail
 
 using PlannerDit64 = detail::PlannerDit<double>;
@@ -302,6 +350,10 @@ using PlannerAny64 = detail::PlannerAny<double>;
 using PlannerAny32 = detail::PlannerAny<float>;
 using PlannerR2cAny64 = detail::PlannerR2cAny<double>;
 using PlannerR2cAny32 = detail::PlannerR2cAny<float>;
+using R2rKind = detail::R2rKind;
+using R2rNorm = detail::R2rNorm;
+using PlannerDct64 = detail::PlannerDct<double>;
+using PlannerDct32 = detail::PlannerDct<float>;
 
 // ---- c2c (lib.rs:143-226, algorithms/dit.rs:263,338): in place on planar vectors -----------------------
 inline void fft_64_dit_with_planner_and_opts(std::vector<double>& reals, std::vector<double>& imags, Direction d, const PlannerDit64& p, const Options&) {

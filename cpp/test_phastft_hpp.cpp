@@ -18,6 +18,7 @@ int main() {
     fails += !panics_with([] { PlannerDit64 p(5); }, "power of two");
     fails += !panics_with([] { PlannerDit32 p(0); }, "power of two");
     fails += !panics_with([] { PlannerR2c64 p(6); }, "n must be a power of 2 >= 4");
+    fails += !panics_with([] { PlannerDct64 p(0); }, "n must be >= 1");
     fails += !panics_with([] { std::vector<float> x(2), a(2), b(2); r2c_fft_f32(x, a, b); }, "n must be a power of 2 >= 4");
     Options o = Options::guess_options(1 << 16);
     fails += !(o.multithreaded_bit_reversal && o.smallest_parallel_chunk_size == 16384);
@@ -46,6 +47,16 @@ int main() {
             fft_32_dit_with_planner(a, c, Direction::Forward, p);
             for (std::size_t i = 0; i < n; ++i) fails += a[i] != bre[b * stride + i] || c[i] != bim[b * stride + i];
         }
+    }
+    {   // additive surface: DCT-II then DCT-III of it, divided by 2N, gives the input back; in place on the host
+        const std::size_t n = 1000;
+        PlannerDct64 p(n);
+        fails += p.n() != n || p.describe().find("n=1000 f64 dct | ") != 0;
+        std::vector<double> x(n), y(n);
+        for (std::size_t i = 0; i < n; ++i) x[i] = std::sin(0.37 * i);
+        p.transform(R2rKind::Dct2, R2rNorm::Backward, x, y);
+        p.transform(R2rKind::Dct3, R2rNorm::Forward, y, y);
+        for (std::size_t i = 0; i < n; ++i) fails += std::fabs(y[i] - x[i]) > 1e-12;
     }
     std::printf("gpu checks: %d failures\n", fails);
     return fails;

@@ -54,7 +54,8 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * C=<members>) and CHIRP-PRE-IL / CHIRP-POST-IL / SMOOTH-PRE-IL / ODD-IL (the complex any-length transform's end kernels, the
  * last ODD pass only, in phastft_fft_interleaved_any_*: R, C and NT as in the planar call), R2C-UNTANGLE-IL / C2R-PRE-IL /
  * CHIRP-POST-R2C-IL / CHIRP-PRE-C2R-IL / SMOOTH-PRE-C2R-IL / ODD-R2C-IL / SMOOTH-POST-R2C-IL (the spectrum's end of
- * phastft_{r2c,c2r}_interleaved_any_*, whose halved mixed r2c's last pass is ODD-IL); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * phastft_{r2c,c2r}_interleaved_any_*, whose halved mixed r2c's last pass is ODD-IL), DCT-PRE-<kind> / DCT-POST-<kind> (the ends of
+ * phastft_dct_*, kind DCT2, DCT3, DST2 or DST3: R=<N>, C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), c2r-in-il (the same from interleaved bins), cluster, pipe or pipe-tma; " pdl" marks
  * programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
@@ -449,6 +450,54 @@ PHASTFT_API int32_t phastft_c2r_interleaved_any_f64_host(const phastft_plan_r2c_
                                                          double* output, size_t len_out);
 PHASTFT_API int32_t phastft_c2r_interleaved_any_f32_host(const phastft_plan_r2c_any_f32* plan, const float* in, size_t len_in_complex,
                                                          float* output, size_t len_out);
+
+/* ---- discrete cosine and sine transforms, types 2 and 3, of any length (scipy.fft.dct / dst) ----------------------------
+ * kind, with N = n and scipy.fft's definitions (norm "backward"):
+ *   PHASTFT_R2R_DCT2  y[k] = 2 sum_n x[n] cos(pi k (2n + 1) / 2N)
+ *   PHASTFT_R2R_DCT3  y[k] = x[0] + 2 sum_{n >= 1} x[n] cos(pi n (2k + 1) / 2N)
+ *   PHASTFT_R2R_DST2  y[k] = 2 sum_n x[n] sin(pi (k + 1)(2n + 1) / 2N)
+ *   PHASTFT_R2R_DST3  y[k] = (-1)^k x[N-1] + 2 sum_{n < N-1} x[n] sin(pi (n + 1)(2k + 1) / 2N)
+ * norm: PHASTFT_NORM_BACKWARD (as above), PHASTFT_NORM_ORTHO (scaled by 1/sqrt(2N), with scipy's orthogonalize=True: output 0
+ * of DCT-II / input 0 of DCT-III scaled by 1/sqrt(2) / sqrt(2), element N-1 for the DSTs), PHASTFT_NORM_FORWARD (1/(2N)).
+ * scipy's idct / idst of type t and norm m is kind t' = 5 - t with the inverse norm (backward <-> forward, ortho itself).
+ * Each call runs DCT-PRE-<kind>, the inner real plan's interleaved r2c (types 2) or c2r (types 3) on the plan's workspace, and
+ * DCT-POST-<kind>.  _create_with takes PHASTFT_ANY_* and has the limits and refusals of phastft_plan_r2c_any_*_create_with;
+ * describe() is "n=<N> <prec> dct | " followed by the inner real plan's describe().
+ * _dev: member b reads N reals at d_in + b * in_stride and writes N reals at d_out + b * out_stride; any strides >= N and any
+ * element offsets (the caller's arrays are accessed one element at a time), d_out == d_in with equal strides transforms in
+ * place.  A bad kind or norm, NULL pointers and short strides return PHASTFT_ERR_INVALID_ARG before any launch; batch == 0 does
+ * nothing.  The workspace follows the any-length plans' protocol: it grows outside a stream capture only (a capture that would
+ * need it to grow returns PHASTFT_ERR_INVALID_ARG; _reserve(batch) grows it and the inner plan's beforehand), and a call on
+ * another stream waits for the previous one.
+ * _host: synchronous, through a plan-owned staging buffer (allocated by the first host call); len_in != N is
+ * PHASTFT_ERR_INPUT_LEN, len_out != N PHASTFT_ERR_OUTPUT_LEN; in may equal out. */
+#define PHASTFT_R2R_DCT2 0
+#define PHASTFT_R2R_DCT3 1
+#define PHASTFT_R2R_DST2 2
+#define PHASTFT_R2R_DST3 3
+#define PHASTFT_NORM_BACKWARD 0
+#define PHASTFT_NORM_ORTHO 1
+#define PHASTFT_NORM_FORWARD 2
+typedef struct phastft_plan_dct_f64 phastft_plan_dct_f64;
+typedef struct phastft_plan_dct_f32 phastft_plan_dct_f32;
+PHASTFT_API int32_t phastft_plan_dct_f64_create_with(size_t n, int device, int algo, phastft_plan_dct_f64** out);
+PHASTFT_API int32_t phastft_plan_dct_f32_create_with(size_t n, int device, int algo, phastft_plan_dct_f32** out);
+PHASTFT_API void phastft_plan_dct_f64_destroy(phastft_plan_dct_f64* plan);
+PHASTFT_API void phastft_plan_dct_f32_destroy(phastft_plan_dct_f32* plan);
+PHASTFT_API size_t phastft_plan_dct_f64_size(const phastft_plan_dct_f64* plan);
+PHASTFT_API size_t phastft_plan_dct_f32_size(const phastft_plan_dct_f32* plan);
+PHASTFT_API const char* phastft_plan_dct_f64_describe(const phastft_plan_dct_f64* plan);
+PHASTFT_API const char* phastft_plan_dct_f32_describe(const phastft_plan_dct_f32* plan);
+PHASTFT_API int32_t phastft_plan_dct_f64_reserve(const phastft_plan_dct_f64* plan, size_t batch);
+PHASTFT_API int32_t phastft_plan_dct_f32_reserve(const phastft_plan_dct_f32* plan, size_t batch);
+PHASTFT_API int32_t phastft_dct_f64_dev(const phastft_plan_dct_f64* plan, int kind, int norm, const double* d_in, size_t in_stride,
+                                        double* d_out, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_dct_f32_dev(const phastft_plan_dct_f32* plan, int kind, int norm, const float* d_in, size_t in_stride,
+                                        float* d_out, size_t out_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_dct_f64_host(const phastft_plan_dct_f64* plan, int kind, int norm, const double* in, size_t len_in,
+                                         double* out, size_t len_out);
+PHASTFT_API int32_t phastft_dct_f32_host(const phastft_plan_dct_f32* plan, int kind, int norm, const float* in, size_t len_in,
+                                         float* out, size_t len_out);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

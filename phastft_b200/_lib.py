@@ -131,6 +131,13 @@ SIGNATURES = {
     "phastft_c2r_interleaved_any_{s}_dev": ([_vp, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
     "phastft_r2c_interleaved_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz], _i32),
     "phastft_c2r_interleaved_any_{s}_host": ([_vp, _vp, _sz, _vp, _sz], _i32),
+    "phastft_plan_dct_{s}_create_with": ([_sz, _ci, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_dct_{s}_destroy": ([_vp], None),
+    "phastft_plan_dct_{s}_size": ([_vp], _sz),
+    "phastft_plan_dct_{s}_describe": ([_vp], C.c_char_p),
+    "phastft_plan_dct_{s}_reserve": ([_vp, _sz], _i32),
+    "phastft_dct_{s}_dev": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_dct_{s}_host": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz], _i32),
 }
 def check(code: int):
     if code != OK:

@@ -46,6 +46,8 @@ __all__ = [
     "r2c_fft_f64_interleaved_any_with_planner", "r2c_fft_f32_interleaved_any_with_planner",
     "c2r_fft_f64_interleaved_any_with_planner", "c2r_fft_f32_interleaved_any_with_planner",
     "r2c_interleaved_any_batch", "c2r_interleaved_any_batch",
+    "PlannerDct64", "PlannerDct32", "dct_f64_with_planner", "dct_f32_with_planner", "dst_f64_with_planner", "dst_f32_with_planner",
+    "dct_batch", "dst_batch",
 ]
 
 
@@ -1041,3 +1043,128 @@ def c2r_interleaved_any_batch(spec, out, planner, batch: int, in_stride: int | N
     """c2r_any_batch from a flat 1-D complex torch CUDA tensor: member b reads N/2 + 1 bins at spec[b * in_stride:] (complex
     values) and writes N reals at out[b * out_stride:] (defaults: N/2 + 1 and N)."""
     _c2r_interleaved_any(planner._sfx, spec, out, planner, int(batch), in_stride, out_stride)
+
+
+# ----------------------------------------------------------------------------------------------
+# discrete cosine and sine transforms, types 2 and 3, of any length (scipy.fft.dct / dst)
+# ----------------------------------------------------------------------------------------------
+class _PlannerDct:
+    _sfx = ""
+    _dtype = None
+
+    def __init__(self, n: int, device: int = 0, algo: AnyAlgo = AnyAlgo.Auto):
+        """DCT / DST types 2 and 3 of length n >= 1 over an n-point real FFT (PlannerR2cAny's, built with `algo`, so with its
+        limits and refusals: PhastFTPanic(13) before the device is touched for n = 0)."""
+        self._h = C.c_void_p()
+        self.device = int(device)
+        check(fn("phastft_plan_dct_{s}_create_with", self._sfx)(int(n), self.device, int(algo), C.byref(self._h)))
+        self.n = int(n)
+
+    def describe(self) -> str:
+        """"n=<N> <prec> dct | " followed by the inner real plan's describe()."""
+        return fn("phastft_plan_dct_{s}_describe", self._sfx)(self._h).decode()
+
+    def reserve(self, batch: int) -> None:
+        """Make every allocation a call of `batch` members would make now (otherwise the first larger call makes them,
+        synchronising the device -- an error inside a CUDA-graph capture)."""
+        check(fn("phastft_plan_dct_{s}_reserve", self._sfx)(self._h, int(batch)))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._h = None
+            try:
+                fn("phastft_plan_dct_{s}_destroy", self._sfx)(h)
+            except (AttributeError, TypeError):      # interpreter shutdown: the module globals are already gone
+                pass
+
+
+class PlannerDct64(_PlannerDct):
+    _sfx, _dtype = "f64", np.float64
+
+
+class PlannerDct32(_PlannerDct):
+    _sfx, _dtype = "f32", np.float32
+
+
+_NORMS = {None: 0, "backward": 0, "ortho": 1, "forward": 2}
+
+
+def _r2r_kind(sine: bool, type, norm):
+    """(kind, norm) codes of include/phastft_cuda.h (PHASTFT_R2R_*, PHASTFT_NORM_*)"""
+    if isinstance(type, bool) or not isinstance(type, (int, np.integer)) or type not in (2, 3):
+        raise ValueError(f"type must be 2 or 3, got {type!r}")
+    if norm not in _NORMS:
+        raise ValueError(f"norm must be 'backward', 'ortho' or 'forward', got {norm!r}")
+    return int(type) - 2 + 2 * sine, _NORMS[norm]
+
+
+def _r2r(sine, x, out, planner, batch, type, norm, in_stride, out_stride):
+    kind, nc = _r2r_kind(sine, type, norm)
+    if not (_is_torch(x) and _is_torch(out)):
+        raise TypeError("expected 1-D torch CUDA tensors (use dct_*_with_planner for numpy arrays)")
+    n = planner.n
+    in_stride = n if in_stride is None else int(in_stride)
+    out_stride = n if out_stride is None else int(out_stride)
+    px, nx = _torch_ptr(x, planner._dtype)
+    po, no = _torch_ptr(out, planner._dtype)
+    _check_batch_len("input", nx, batch, in_stride, n)
+    _check_batch_len("output", no, batch, out_stride, n)
+    check(fn("phastft_dct_{s}_dev", planner._sfx)(planner._h, kind, nc, px, in_stride, po, out_stride, int(batch), _torch_stream(x)))
+
+
+def _r2r_with_planner(sfx, sine, x, out, planner, type, norm):
+    if planner._sfx != sfx:
+        raise TypeError("planner precision does not match the function")
+    kind, nc = _r2r_kind(sine, type, norm)
+    if _is_torch(x) != _is_torch(out):
+        raise TypeError("pass the input and the output both as numpy arrays or both as torch CUDA tensors")
+    if _is_torch(x):
+        _torch_ptr(x, planner._dtype)
+        _torch_ptr(out, planner._dtype)
+        if x.numel() != planner.n:
+            raise PhastFTPanic(5)
+        if out.numel() != planner.n:
+            raise PhastFTPanic(8)
+        _r2r(sine, x, out, planner, 1, type, norm, None, None)
+        return
+    px, nx = _np_ptr(x, planner._dtype, False)
+    po, no = _np_ptr(out, planner._dtype, True)
+    if nx != planner.n:
+        raise PhastFTPanic(5)
+    if no != planner.n:
+        raise PhastFTPanic(8)
+    check(fn("phastft_dct_{s}_host", sfx)(planner._h, kind, nc, px, nx, po, no))
+
+
+def dct_f64_with_planner(x, out, planner: PlannerDct64, type: int = 2, norm: str = "backward") -> None:
+    """scipy.fft.dct(x, type, norm=norm) of N = planner.n values into out: float64 numpy arrays (synchronous) or 1-D torch CUDA
+    tensors (torch's current stream).  out may be x.  scipy.fft.idct(X, type=2, norm=m) is type=3 with the inverse norm
+    ("backward" <-> "forward", "ortho" itself), and idct of type 3 is type 2."""
+    _r2r_with_planner("f64", False, x, out, planner, type, norm)
+
+
+def dct_f32_with_planner(x, out, planner: PlannerDct32, type: int = 2, norm: str = "backward") -> None:
+    _r2r_with_planner("f32", False, x, out, planner, type, norm)
+
+
+def dst_f64_with_planner(x, out, planner: PlannerDct64, type: int = 2, norm: str = "backward") -> None:
+    """scipy.fft.dst(x, type, norm=norm), as dct_f64_with_planner."""
+    _r2r_with_planner("f64", True, x, out, planner, type, norm)
+
+
+def dst_f32_with_planner(x, out, planner: PlannerDct32, type: int = 2, norm: str = "backward") -> None:
+    _r2r_with_planner("f32", True, x, out, planner, type, norm)
+
+
+def dct_batch(x, out, planner, batch: int, type: int = 2, norm: str = "backward", in_stride: int | None = None,
+              out_stride: int | None = None) -> None:
+    """`batch` DCTs on flat 1-D torch CUDA tensors: member b reads N values at x[b * in_stride:] and writes N at
+    out[b * out_stride:] (defaults: N; any strides >= N, any offsets; out may be x with equal strides)."""
+    _r2r(False, x, out, planner, int(batch), type, norm, in_stride, out_stride)
+
+
+def dst_batch(x, out, planner, batch: int, type: int = 2, norm: str = "backward", in_stride: int | None = None,
+              out_stride: int | None = None) -> None:
+    """dct_batch for the DST."""
+    _r2r(True, x, out, planner, int(batch), type, norm, in_stride, out_stride)

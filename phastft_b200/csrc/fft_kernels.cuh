@@ -1585,4 +1585,80 @@ __global__ void __launch_bounds__(256) smooth_post_r2c_kernel(const __grid_const
     if (m != k) y.put(m, xm.x, xm.y);
 }
 
+// ---------------------------------------------------------------------------------------------
+// DCT-PRE / DCT-POST: the two elementwise ends of the DCT / DST types 2 and 3 over an N-point real FFT (Makhoul 1980), with
+// W = W_(4N) from a two-level table.  DCT-II: v[n] = x[2n], v[N-1-n] = x[2n+1]; V = rfft(v); u = W^k V[k],
+// y[k] = 2 Re u, y[N-k] = -2 Im u.  DCT-III: bin k = W^-k (x[k] - i x[N-k]) (x[N] = 0); v = irfft(bins) * N;
+// y[2n] = v[n], y[2n+1] = v[N-1-n].  DST-II is DCT-II of (-1)^n x[n] with the output reversed, DST-III (-1)^k DCT-III of x
+// reversed: the DST kinds negate the odd-indexed side of the permutation and reverse the caller's side of the twiddle.  The
+// norm is folded into `scale` (and the ortho factor into `scale0`, for output 0 of DCT-II / input 0 of DCT-III, i.e. element
+// N-1 of a DST), the c2r's 1/N into DCT-III's scale.  The caller's arrays (`re`, any stride and offset) are read or written with
+// scalar accesses only; the workspace's reals `v` (even stride) and bins (one complex access each) belong to the plan.
+// One thread per (n, N-1-n) pair (the permutations) or per bin k <= N/2 (the twiddles); a member-major grid of 256-thread
+// blocks.
+enum DctKind { DCT_KIND_DCT2 = 0, DCT_KIND_DCT3 = 1, DCT_KIND_DST2 = 2, DCT_KIND_DST3 = 3 };
+template <typename T>
+struct DctParams {
+    const T* in;                   // the caller's input (PRE) or the workspace reals (type 3's POST)
+    T* out;                        // the workspace reals (type 2's PRE) or the caller's output (POST)
+    cx<T>* bins;                   // the workspace bins, floor(N/2) + 1 per member
+    const cx<T>* w_hi;             // W_(4N)^e = w_hi[e >> lo_bits] w_lo[e & (2^lo_bits - 1)]
+    const cx<T>* w_lo;
+    long long n, in_stride, out_stride, bin_stride;   // member strides: T, T, complex values
+    T scale, scale0;
+    int lo_bits;
+    unsigned blocks_per_member;
+};
+
+// v[n] = x[2n], v[N-1-n] = +-x[2n+1] (type 2's PRE), or its inverse y[2n] = v[n], y[2n+1] = +-v[N-1-n] (type 3's POST)
+template <typename T, bool DST, bool INVERSE>
+__device__ __forceinline__ void dct_permute(const DctParams<T>& p, long long mb, long long j) {
+    if (2 * j >= p.n) return;
+    const T* x = p.in + mb * p.in_stride;
+    T* y = p.out + mb * p.out_stride;
+    const long long r = p.n - 1 - j;
+    if constexpr (INVERSE) {
+        y[2 * j] = x[j];
+        if (2 * j + 1 < p.n) y[2 * j + 1] = DST ? -x[r] : x[r];
+    } else {
+        y[j] = x[2 * j];
+        if (2 * j + 1 < p.n) y[r] = DST ? -x[2 * j + 1] : x[2 * j + 1];
+    }
+}
+
+template <typename T, int KIND>
+__global__ void __launch_bounds__(256) dct_pre_kernel(const __grid_constant__ DctParams<T> p) {
+    constexpr bool DST = KIND == DCT_KIND_DST2 || KIND == DCT_KIND_DST3;
+    const unsigned mb = blockIdx.x / p.blocks_per_member;
+    const long long j = (long long)(blockIdx.x - mb * p.blocks_per_member) * 256 + threadIdx.x;
+    if constexpr (KIND == DCT_KIND_DCT2 || KIND == DCT_KIND_DST2) {
+        dct_permute<T, DST, false>(p, mb, j);
+    } else {
+        if (2 * j > p.n) return;
+        const T* x = p.in + (long long)mb * p.in_stride;
+        // x[k] and x[N-k] of the DCT-III input, x reversed for DST-III
+        const T a = x[DST ? p.n - 1 - j : j] * (j ? p.scale : p.scale0);
+        const T b = j ? x[DST ? j - 1 : p.n - j] * p.scale : T(0);
+        const cx<T> w = two_level_root<T>(p.w_hi, p.w_lo, p.lo_bits, (unsigned long long)j);
+        p.bins[(long long)mb * p.bin_stride + j] = cmul<T>(make_cx<T>(w.x, -w.y), make_cx<T>(a, -b));
+    }
+}
+
+template <typename T, int KIND>
+__global__ void __launch_bounds__(256) dct_post_kernel(const __grid_constant__ DctParams<T> p) {
+    constexpr bool DST = KIND == DCT_KIND_DST2 || KIND == DCT_KIND_DST3;
+    const unsigned mb = blockIdx.x / p.blocks_per_member;
+    const long long k = (long long)(blockIdx.x - mb * p.blocks_per_member) * 256 + threadIdx.x;
+    if constexpr (KIND == DCT_KIND_DCT3 || KIND == DCT_KIND_DST3) {
+        dct_permute<T, DST, true>(p, mb, k);
+    } else {
+        if (2 * k > p.n) return;
+        const cx<T> u = cmul<T>(two_level_root<T>(p.w_hi, p.w_lo, p.lo_bits, (unsigned long long)k), p.bins[(long long)mb * p.bin_stride + k]);
+        T* y = p.out + (long long)mb * p.out_stride;
+        // DCT-II outputs k and N-k; DST-II stores output j of the DCT at N-1-j
+        y[DST ? p.n - 1 - k : k] = u.x * (k ? p.scale : p.scale0);
+        if (k && 2 * k != p.n) y[DST ? k - 1 : p.n - k] = -u.y * p.scale;
+    }
+}
+
 }  // namespace phast

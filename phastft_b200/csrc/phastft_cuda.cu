@@ -3569,6 +3569,158 @@ int32_t c2r_any_host(const PlanR2cAny<T>* pl, const T* ire, size_t len_ire, cons
     return PHASTFT_OK;
 }
 
+// =================================================================================================
+// DCT / DST types 2 and 3 of any length: DCT-PRE, the real any-length plan's interleaved r2c (type 2) or c2r (type 3) on the
+// plan's workspace, DCT-POST (fft_kernels.cuh, Makhoul 1980)
+// =================================================================================================
+template <typename T>
+struct PlanDct {
+    size_t n = 0;
+    int device = 0;
+    PlanR2cAny<T>* inner = nullptr;    // the N-point real plan
+    TwoLevelRoots<T> w4n;              // W_(4N)^k for k <= N/2
+    // per call of `batch` members: batch x vstride() reals v, then batch x (N/2 + 1) bins; the AnyWorkspace protocol
+    mutable AnyWorkspace<T> w;
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then w.mu, then the inner plan's)
+    mutable T* stage = nullptr;        // host-API staging: N reals, transformed in place; allocated by the first host call
+    std::string description;
+    size_t vstride() const { return n + (n & 1); }                 // even, so the inner r2c may read v as pairs
+    size_t member_elems() const { return vstride() / 2 + n / 2 + 1; }   // complex values
+    cudaStream_t host_stream() const { return inner->pow2 ? inner->pow2->inner->stream : inner->host_stream(); }
+    ~PlanDct() {
+        DeviceGuard g(device);
+        w.destroy();
+        if (w4n.blob) cudaFree(w4n.blob);
+        if (stage) cudaFree(stage);
+        delete inner;
+    }
+};
+
+template <typename T>
+int32_t build_plan_dct(size_t n, int device, int algo, PlanDct<T>** out) {
+    if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
+    *out = nullptr;
+    if (n == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n must be >= 1");
+    std::unique_ptr<PlanDct<T>> pl(new PlanDct<T>());
+    pl->n = n; pl->device = device;
+    if (int32_t st = build_plan_r2c_any<T>(n, device, algo, &pl->inner)) return st;
+    DeviceGuard g(device);
+    if (int32_t st = build_two_level(pl->w4n, 4 * n, n / 2 + 1)) return st;
+    if (int32_t st = pl->w.init(pl->member_elems())) return st;   // room for one member; batched calls grow it
+    pl->description = "n=" + std::to_string(n) + (sizeof(T) == 8 ? " f64" : " f32") + " dct | ";
+    *out = pl.release();
+    return PHASTFT_OK;
+}
+
+template <typename T>
+std::string dct_description(const PlanDct<T>* pl) { return pl->description + r2c_any_description(pl->inner); }
+
+template <typename T>
+int32_t dct_reserve(const PlanDct<T>* pl, size_t batch) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (int32_t st = r2c_any_reserve(pl->inner, batch)) return st;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    return pl->w.grow(batch * pl->member_elems(), batch);
+}
+
+// One DCT-PRE or DCT-POST over `batch` members, in launches of at most 2^31 - 1 blocks.  Launch record: R = N, C = the members
+// of that launch.
+template <typename T>
+int32_t launch_dct_end(bool post, int kind, DctParams<T> p, size_t threads, size_t batch, cudaStream_t stream) {
+    static const char* const names[2][4] = {{"DCT-PRE-DCT2", "DCT-PRE-DCT3", "DCT-PRE-DST2", "DCT-PRE-DST3"},
+                                             {"DCT-POST-DCT2", "DCT-POST-DCT3", "DCT-POST-DST2", "DCT-POST-DST3"}};
+    const size_t bpm = (threads + 255) / 256;
+    p.blocks_per_member = (unsigned)bpm;
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    for (size_t done = 0; done < batch; done += max_members) {
+        const size_t nb = std::min(batch - done, max_members);
+        DctParams<T> q = p;
+        q.in += done * p.in_stride;
+        q.out += done * p.out_stride;
+        q.bins += done * p.bin_stride;
+        launch_dct<T>(post, kind, q, (unsigned)(nb * bpm), stream);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({names[post][kind], (int)std::min<size_t>(p.n, INT32_MAX), 0, (int)nb, 256, 0, "plain", false});
+    }
+    return PHASTFT_OK;
+}
+
+// Member b reads N reals at d_in + b * in_stride and writes N reals at d_out + b * out_stride (any strides >= N, any element
+// offsets, d_out == d_in with equal strides in place).  kind PHASTFT_R2R_*, norm PHASTFT_NORM_* with scipy.fft's meanings.
+template <typename T>
+int32_t dct_dev(const PlanDct<T>* pl, int kind, int norm, const T* d_in, size_t in_stride, T* d_out, size_t out_stride, size_t batch,
+                cudaStream_t stream) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (kind < PHASTFT_R2R_DCT2 || kind > PHASTFT_R2R_DST3)
+        return fail(PHASTFT_ERR_INVALID_ARG, "kind must be PHASTFT_R2R_DCT2, _DCT3, _DST2 or _DST3");
+    if (norm < PHASTFT_NORM_BACKWARD || norm > PHASTFT_NORM_FORWARD)
+        return fail(PHASTFT_ERR_INVALID_ARG, "norm must be PHASTFT_NORM_BACKWARD, _ORTHO or _FORWARD");
+    if (!d_in) return fail(PHASTFT_ERR_INVALID_ARG, "d_in == NULL");
+    if (!d_out) return fail(PHASTFT_ERR_INVALID_ARG, "d_out == NULL");
+    const size_t n = pl->n, bins = n / 2 + 1, vs = pl->vstride();
+    if (in_stride < n) return fail(PHASTFT_ERR_INVALID_ARG, "in_stride must be >= N = " + std::to_string(n) + " (got " + std::to_string(in_stride) + ")");
+    if (out_stride < n) return fail(PHASTFT_ERR_INVALID_ARG, "out_stride must be >= N = " + std::to_string(n) + " (got " + std::to_string(out_stride) + ")");
+    if (batch == 0) return PHASTFT_OK;
+    const bool type2 = kind == PHASTFT_R2R_DCT2 || kind == PHASTFT_R2R_DST2;
+    // scipy's norms: type 2 y = 2 c sum(...), type 3 y = c (x[0] + 2 sum(...)), c = 1, 1/sqrt(2N) or 1/(2N); ortho also scales
+    // output 0 of type 2 by 1/sqrt(2) and input 0 of type 3 by sqrt(2) (element N-1 for DST).  Type 3 also undoes the c2r's 1/N.
+    const long double c = norm == PHASTFT_NORM_BACKWARD ? 1.0L : norm == PHASTFT_NORM_ORTHO ? 1.0L / sqrtl(2.0L * n) : 1.0L / (2.0L * n);
+    const long double s = type2 ? 2.0L * c : (long double)n * c;
+    const long double s0 = norm != PHASTFT_NORM_ORTHO ? s : type2 ? s / sqrtl(2.0L) : s * sqrtl(2.0L);
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    bool capturing = false;
+    if (int32_t st = pl->w.acquire(batch * pl->member_elems(), batch, stream, "phastft_plan_dct_*_reserve", capturing)) return st;
+    T* v = reinterpret_cast<T*>(pl->w.ws);
+    cx<T>* spec = pl->w.ws + batch * vs / 2;
+    DctParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.bins = spec; p.bin_stride = (long long)bins;
+    p.w_hi = pl->w4n.hi; p.w_lo = pl->w4n.lo; p.lo_bits = pl->w4n.lo_bits;
+    p.n = (long long)n; p.scale = (T)s; p.scale0 = (T)s0;
+    // type 2: x -> v (pairs), r2c, bins -> y (bins); type 3: x -> bins (bins), c2r, v -> y (pairs)
+    DctParams<T> pre = p, post = p;
+    pre.in = d_in; pre.in_stride = (long long)in_stride;
+    post.out = d_out; post.out_stride = (long long)out_stride;
+    if (type2) { pre.out = v; pre.out_stride = (long long)vs; }
+    else { post.in = v; post.in_stride = (long long)vs; }
+    const size_t pairs = (n + 1) / 2;
+    int32_t st = launch_dct_end<T>(false, kind, pre, type2 ? pairs : bins, batch, stream);
+    if (!st) st = type2 ? r2c_il_any_dev(pl->inner, v, vs, reinterpret_cast<T*>(spec), bins, batch, stream)
+                        : c2r_il_any_dev(pl->inner, reinterpret_cast<const T*>(spec), bins, v, vs, batch, stream);
+    if (!st) st = launch_dct_end<T>(true, kind, post, type2 ? bins : pairs, batch, stream);
+    const int32_t rel = pl->w.release(stream, capturing);   // also after a failed launch: the kernels queued so far used it
+    return st ? st : rel;
+}
+
+// host slices, synchronous: the N reals are staged through one plan-owned buffer and transformed in place there
+template <typename T>
+int32_t dct_host(const PlanDct<T>* pl, int kind, int norm, const T* in, size_t len_in, T* out, size_t len_out) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (kind < PHASTFT_R2R_DCT2 || kind > PHASTFT_R2R_DST3)
+        return fail(PHASTFT_ERR_INVALID_ARG, "kind must be PHASTFT_R2R_DCT2, _DCT3, _DST2 or _DST3");
+    if (norm < PHASTFT_NORM_BACKWARD || norm > PHASTFT_NORM_FORWARD)
+        return fail(PHASTFT_ERR_INVALID_ARG, "norm must be PHASTFT_NORM_BACKWARD, _ORTHO or _FORWARD");
+    const size_t n = pl->n;
+    if (len_in != n) return fail(PHASTFT_ERR_INPUT_LEN);
+    if (len_out != n) return fail(PHASTFT_ERR_OUTPUT_LEN);
+    if (!in || !out) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->host_stream();
+    {
+        std::lock_guard<std::mutex> lock(pl->w.mu);   // released before the device call, which takes it
+        if (!pl->stage) CUDA_TRY(cudaMalloc(&pl->stage, n * sizeof(T)));
+    }
+    CUDA_TRY(scribble(pl->w.scribble_on, pl->stage, n * sizeof(T), s));
+    CUDA_TRY(cudaMemcpyAsync(pl->stage, in, n * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = dct_dev(pl, kind, norm, pl->stage, n, pl->stage, n, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(out, pl->stage, n * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -3582,6 +3734,8 @@ int32_t c2r_any_host(const PlanR2cAny<T>* pl, const T* ire, size_t len_ire, cons
 #define AS_CANY(T, p) reinterpret_cast<const PlanAny<T>*>(p)
 #define AS_R2CANY(T, p) reinterpret_cast<PlanR2cAny<T>*>(p)
 #define AS_CR2CANY(T, p) reinterpret_cast<const PlanR2cAny<T>*>(p)
+#define AS_DCT(T, p) reinterpret_cast<PlanDct<T>*>(p)
+#define AS_CDCT(T, p) reinterpret_cast<const PlanDct<T>*>(p)
 
 extern "C" {
 
@@ -3910,6 +4064,33 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                          size_t liim, T* out, size_t lout) {                                            \
         launches_reset();                                                                                               \
         return c2r_any_host<T>(AS_CR2CANY(T, p), ire, lire, iim, liim, out, lout);                                      \
+    }                                                                                                                   \
+    int32_t phastft_plan_dct_##SFX##_create_with(size_t n, int device, int algo, phastft_plan_dct_##SFX** out) {        \
+        PlanDct<T>* pl = nullptr;                                                                                       \
+        int32_t st = build_plan_dct<T>(n, device, algo, &pl);                                                           \
+        if (out) *out = reinterpret_cast<phastft_plan_dct_##SFX*>(pl);                                                  \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    void phastft_plan_dct_##SFX##_destroy(phastft_plan_dct_##SFX* p) { delete AS_DCT(T, p); }                           \
+    size_t phastft_plan_dct_##SFX##_size(const phastft_plan_dct_##SFX* p) { return p ? AS_CDCT(T, p)->n : 0; }          \
+    const char* phastft_plan_dct_##SFX##_describe(const phastft_plan_dct_##SFX* p) {                                    \
+        if (!p) return "";                                                                                              \
+        g_r2c_desc_text = dct_description<T>(AS_CDCT(T, p));                                                            \
+        return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
+    int32_t phastft_plan_dct_##SFX##_reserve(const phastft_plan_dct_##SFX* p, size_t batch) {                           \
+        return dct_reserve<T>(AS_CDCT(T, p), batch);                                                                    \
+    }                                                                                                                   \
+    int32_t phastft_dct_##SFX##_dev(const phastft_plan_dct_##SFX* p, int kind, int norm, const T* in, size_t in_stride,  \
+                                    T* out, size_t out_stride, size_t batch, void* s) {                                 \
+        launches_reset();                                                                                               \
+        return dct_dev<T>(AS_CDCT(T, p), kind, norm, in, in_stride, out, out_stride, batch, (cudaStream_t)s);           \
+    }                                                                                                                   \
+    int32_t phastft_dct_##SFX##_host(const phastft_plan_dct_##SFX* p, int kind, int norm, const T* in, size_t lin,       \
+                                     T* out, size_t lout) {                                                             \
+        launches_reset();                                                                                               \
+        return dct_host<T>(AS_CDCT(T, p), kind, norm, in, lin, out, lout);                                              \
     }
 
 DEFINE_DIT_API(double, f64)

@@ -134,4 +134,7 @@ template <typename T> void launch_smooth_pre_real_il(int mode, const SmoothParam
 template <typename T> bool launch_odd_r2c_il(const OddParams<T>& q, int r, size_t smem, unsigned grid, cudaStream_t stream);
 template <typename T> void launch_smooth_post_r2c_il(const SmoothPostParams<T>& p, unsigned grid, cudaStream_t stream);
 
+// defined in r2r.cu: DCT-PRE (`post` false) or DCT-POST of DctKind `kind`
+template <typename T> void launch_dct(bool post, int kind, const DctParams<T>& p, unsigned grid, cudaStream_t stream);
+
 }  // namespace phast

@@ -20,7 +20,8 @@ pub mod options;
 pub mod planner;
 
 use options::Options;
-use planner::{Direction, PlannerAny32, PlannerAny64, PlannerDit32, PlannerDit64, PlannerR2c32, PlannerR2c64, PlannerR2cAny32, PlannerR2cAny64};
+use planner::{Direction, PlannerAny32, PlannerAny64, PlannerDit32, PlannerDit64, PlannerDct32, PlannerDct64, PlannerR2c32, PlannerR2c64, PlannerR2cAny32,
+              PlannerR2cAny64};
 
 /// Reference panic texts by status code (include/phastft_status.h).
 #[track_caller]
@@ -282,6 +283,47 @@ impl_r2c_any!(r2c_fft_f64_any_with_planner, c2r_fft_f64_any_with_planner, r2c_ff
               f64, PlannerR2cAny64, phastft_r2c_any_f64_host, phastft_c2r_any_f64_host, phastft_r2c_any_f64_dev, phastft_c2r_any_f64_dev);
 impl_r2c_any!(r2c_fft_f32_any_with_planner, c2r_fft_f32_any_with_planner, r2c_fft_f32_any_device_batch, c2r_fft_f32_any_device_batch,
               f32, PlannerR2cAny32, phastft_r2c_any_f32_host, phastft_c2r_any_f32_host, phastft_r2c_any_f32_dev, phastft_c2r_any_f32_dev);
+
+// ------------------------------------------------------------------------------------------------
+// Additive: DCT / DST types 2 and 3 of any length (scipy.fft.dct / dst)
+// ------------------------------------------------------------------------------------------------
+/// The transforms of `PlannerDct*`, with scipy.fft's definitions; `Dct3` with the inverse norm is scipy's idct of type 2.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum R2rKind {
+    Dct2 = 0,
+    Dct3 = 1,
+    Dst2 = 2,
+    Dst3 = 3,
+}
+/// scipy.fft's `norm`: no scale, 1/sqrt(2N) with the orthogonalising factor on the first (DCT) or last (DST) element, or 1/(2N).
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum R2rNorm {
+    Backward = 0,
+    Ortho = 1,
+    Forward = 2,
+}
+macro_rules! impl_dct {
+    ($host:ident, $dev:ident, $t:ty, $planner:ident, $ffi_host:ident, $ffi_dev:ident) => {
+        /// `planner.n()` reals in, as many out.  Panics on a length mismatch.
+        pub fn $host(kind: R2rKind, norm: R2rNorm, input: &[$t], output: &mut [$t], planner: &$planner) {
+            check(unsafe { ffi::$ffi_host(planner.raw, kind as i32, norm as i32, input.as_ptr(), input.len(), output.as_mut_ptr(),
+                                          output.len()) });
+        }
+        /// `batch` transforms on device data: member b reads n reals at `d_in + b * in_stride` and writes n at
+        /// `d_out + b * out_stride` (any strides >= n and offsets; `d_out == d_in` with equal strides in place), stream-ordered.
+        ///
+        /// # Safety
+        /// The pointers must be device pointers valid for the members on the planner's device.
+        pub unsafe fn $dev(kind: R2rKind, norm: R2rNorm, d_in: *const $t, in_stride: usize, d_out: *mut $t, out_stride: usize,
+                           planner: &$planner, batch: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$ffi_dev(planner.raw, kind as i32, norm as i32, d_in, in_stride, d_out, out_stride, batch, stream));
+        }
+    };
+}
+impl_dct!(dct_f64_with_planner, dct_f64_device_batch, f64, PlannerDct64, phastft_dct_f64_host, phastft_dct_f64_dev);
+impl_dct!(dct_f32_with_planner, dct_f32_device_batch, f32, PlannerDct32, phastft_dct_f32_host, phastft_dct_f32_dev);
 
 // ------------------------------------------------------------------------------------------------
 // r2c / c2r  (algorithms/r2c.rs:521-895)

@@ -206,3 +206,43 @@ impl_planner_r2c_any!(PlannerR2cAny64, ffi::phastft_plan_r2c_any_f64, phastft_pl
 impl_planner_r2c_any!(PlannerR2cAny32, ffi::phastft_plan_r2c_any_f32, phastft_plan_r2c_any_f32_create,
                       phastft_plan_r2c_any_f32_create_with, phastft_plan_r2c_any_f32_destroy,
                       phastft_plan_r2c_any_f32_size, phastft_plan_r2c_any_f32_describe, phastft_plan_r2c_any_f32_reserve);
+
+macro_rules! impl_planner_dct {
+    ($name:ident, $raw:ty, $create_with:ident, $destroy:ident, $size:ident, $describe:ident, $reserve:ident) => {
+        /// Additive: DCT / DST types 2 and 3 of any length (scipy.fft.dct / dst) over an N-point real plan.
+        pub struct $name {
+            pub(crate) raw: *mut $raw,
+        }
+        unsafe impl Send for $name {}
+        unsafe impl Sync for $name {}
+        impl $name {
+            /// `algo` as for `PlannerR2cAny*::with_algo`, with its limits.  Panics for `n == 0` or a length above them.
+            pub fn new(n: usize, algo: AnyAlgo) -> Self {
+                let mut raw = std::ptr::null_mut();
+                check(unsafe { ffi::$create_with(n, device(), algo as std::os::raw::c_int, &mut raw) });
+                Self { raw }
+            }
+            /// Number of points the planner was built for.
+            pub fn n(&self) -> usize {
+                unsafe { ffi::$size(self.raw) }
+            }
+            /// `"n=<N> f64 dct | "` followed by the inner real plan's describe().
+            pub fn describe(&self) -> String {
+                unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
+            }
+            /// Makes every allocation a call of `batch` members would make, so such calls can be captured in a CUDA graph.
+            pub fn reserve(&self, batch: usize) {
+                check(unsafe { ffi::$reserve(self.raw, batch) });
+            }
+        }
+        impl Drop for $name {
+            fn drop(&mut self) {
+                unsafe { ffi::$destroy(self.raw) }
+            }
+        }
+    };
+}
+impl_planner_dct!(PlannerDct64, ffi::phastft_plan_dct_f64, phastft_plan_dct_f64_create_with, phastft_plan_dct_f64_destroy,
+                  phastft_plan_dct_f64_size, phastft_plan_dct_f64_describe, phastft_plan_dct_f64_reserve);
+impl_planner_dct!(PlannerDct32, ffi::phastft_plan_dct_f32, phastft_plan_dct_f32_create_with, phastft_plan_dct_f32_destroy,
+                  phastft_plan_dct_f32_size, phastft_plan_dct_f32_describe, phastft_plan_dct_f32_reserve);
