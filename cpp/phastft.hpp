@@ -102,6 +102,14 @@ template <> struct Api<double> {
     static int32_t dct_reserve(const Dct* p, std::size_t b) { return phastft_plan_dct_f64_reserve(p, b); }
     static int32_t dct_dev(const Dct* p, int k, int nm, const double* in, std::size_t is, double* out, std::size_t os, std::size_t b, void* s) { return phastft_dct_f64_dev(p, k, nm, in, is, out, os, b, s); }
     static int32_t dct_host(const Dct* p, int k, int nm, const double* in, std::size_t li, double* out, std::size_t lo) { return phastft_dct_f64_host(p, k, nm, in, li, out, lo); }
+    using Conv = phastft_plan_conv_f64;
+    static int32_t conv_create(std::size_t nx, std::size_t nh, int dom, int dev, Conv** o) { return phastft_plan_conv_f64_create(nx, nh, dom, dev, o); }
+    static void conv_destroy(Conv* p) { phastft_plan_conv_f64_destroy(p); }
+    static std::size_t conv_fft_len(const Conv* p) { return phastft_plan_conv_f64_fft_len(p); }
+    static const char* conv_describe(const Conv* p) { return phastft_plan_conv_f64_describe(p); }
+    static int32_t conv_reserve(const Conv* p, std::size_t b) { return phastft_plan_conv_f64_reserve(p, b); }
+    static int32_t conv_dev(const Conv* p, int op, int m, const double* x, std::size_t xs, const double* h, std::size_t hs, double* y, std::size_t ys, std::size_t b, void* s) { return phastft_conv_f64_dev(p, op, m, x, xs, h, hs, y, ys, b, s); }
+    static int32_t conv_host(const Conv* p, int op, int m, const double* x, std::size_t lx, const double* h, std::size_t lh, double* y, std::size_t ly) { return phastft_conv_f64_host(p, op, m, x, lx, h, lh, y, ly); }
 };
 template <> struct Api<float> {
     using Dit = phastft_plan_dit_f32; using R2c = phastft_plan_r2c_f32;
@@ -155,6 +163,14 @@ template <> struct Api<float> {
     static int32_t dct_reserve(const Dct* p, std::size_t b) { return phastft_plan_dct_f32_reserve(p, b); }
     static int32_t dct_dev(const Dct* p, int k, int nm, const float* in, std::size_t is, float* out, std::size_t os, std::size_t b, void* s) { return phastft_dct_f32_dev(p, k, nm, in, is, out, os, b, s); }
     static int32_t dct_host(const Dct* p, int k, int nm, const float* in, std::size_t li, float* out, std::size_t lo) { return phastft_dct_f32_host(p, k, nm, in, li, out, lo); }
+    using Conv = phastft_plan_conv_f32;
+    static int32_t conv_create(std::size_t nx, std::size_t nh, int dom, int dev, Conv** o) { return phastft_plan_conv_f32_create(nx, nh, dom, dev, o); }
+    static void conv_destroy(Conv* p) { phastft_plan_conv_f32_destroy(p); }
+    static std::size_t conv_fft_len(const Conv* p) { return phastft_plan_conv_f32_fft_len(p); }
+    static const char* conv_describe(const Conv* p) { return phastft_plan_conv_f32_describe(p); }
+    static int32_t conv_reserve(const Conv* p, std::size_t b) { return phastft_plan_conv_f32_reserve(p, b); }
+    static int32_t conv_dev(const Conv* p, int op, int m, const float* x, std::size_t xs, const float* h, std::size_t hs, float* y, std::size_t ys, std::size_t b, void* s) { return phastft_conv_f32_dev(p, op, m, x, xs, h, hs, y, ys, b, s); }
+    static int32_t conv_host(const Conv* p, int op, int m, const float* x, std::size_t lx, const float* h, std::size_t lh, float* y, std::size_t ly) { return phastft_conv_f32_host(p, op, m, x, lx, h, lh, y, ly); }
 };
 
 /// planner.rs:34-114
@@ -339,6 +355,76 @@ class PlannerDct {
   private:
     typename Api<T>::Dct* raw_ = nullptr;
 };
+
+/// additive: linear convolution and cross-correlation (scipy.signal.fftconvolve / correlate) of n_x values with n_h values,
+/// real or complex, over an L-point transform, L = 2^ceil(log2(n_x + n_h - 1)) but at least 4
+enum class ConvMode : int { Full = PHASTFT_CONV_FULL, Same = PHASTFT_CONV_SAME, Valid = PHASTFT_CONV_VALID };
+inline std::size_t conv_out_len(std::size_t n_x, std::size_t n_h, ConvMode mode) { return phastft_conv_out_len(n_x, n_h, static_cast<int>(mode)); }
+template <typename T>
+class PlannerConv {
+  public:
+    /// `complex_domain`: the operands are std::complex<T> (interleaved (re, im) pairs)
+    PlannerConv(std::size_t n_x, std::size_t n_h, int device = 0, bool complex_domain = false) : n_x_(n_x), n_h_(n_h), cplx_(complex_domain) {
+        check(Api<T>::conv_create(n_x, n_h, complex_domain ? PHASTFT_CONV_COMPLEX : PHASTFT_CONV_REAL, device, &raw_));
+    }
+    ~PlannerConv() { if (raw_) Api<T>::conv_destroy(raw_); }
+    PlannerConv(PlannerConv&& o) noexcept : raw_(o.raw_), n_x_(o.n_x_), n_h_(o.n_h_), cplx_(o.cplx_) { o.raw_ = nullptr; }
+    PlannerConv(const PlannerConv&) = delete;
+    PlannerConv& operator=(const PlannerConv&) = delete;
+    std::size_t n_x() const { return n_x_; }
+    std::size_t n_h() const { return n_h_; }
+    bool complex_domain() const { return cplx_; }
+    std::size_t fft_len() const { return Api<T>::conv_fft_len(raw_); }
+    std::size_t out_len(ConvMode mode) const { return conv_out_len(n_x_, n_h_, mode); }
+    /// "n_x=<n_x> n_h=<n_h> <prec> conv <real|complex> L=2^<k> | " followed by the inner plan's description
+    std::string describe() const { return Api<T>::conv_describe(raw_); }
+    /// make every allocation a call of `batch` pairwise members would make now
+    void reserve(std::size_t batch) const { check(Api<T>::conv_reserve(raw_, batch)); }
+    /// real operands on host vectors: y gets the mode's window (y.size() == out_len(mode)).  Throws Panic on a length
+    /// mismatch, and when the planner was built for complex operands (the library would read and write twice the vectors).
+    void convolve(const std::vector<T>& x, const std::vector<T>& h, std::vector<T>& y, ConvMode mode = ConvMode::Full) const {
+        check_domain(false);
+        check(Api<T>::conv_host(raw_, PHASTFT_CONV_CONVOLVE, static_cast<int>(mode), x.data(), x.size(), h.data(), h.size(), y.data(), y.size()));
+    }
+    void correlate(const std::vector<T>& x, const std::vector<T>& h, std::vector<T>& y, ConvMode mode = ConvMode::Full) const {
+        check_domain(false);
+        check(Api<T>::conv_host(raw_, PHASTFT_CONV_CORRELATE, static_cast<int>(mode), x.data(), x.size(), h.data(), h.size(), y.data(), y.size()));
+    }
+    /// complex operands on host vectors; throws Panic when the planner was built for real operands
+    void convolve(const std::vector<std::complex<T>>& x, const std::vector<std::complex<T>>& h, std::vector<std::complex<T>>& y,
+                  ConvMode mode = ConvMode::Full) const {
+        check_domain(true);
+        check(Api<T>::conv_host(raw_, PHASTFT_CONV_CONVOLVE, static_cast<int>(mode), reinterpret_cast<const T*>(x.data()), x.size(),
+                                reinterpret_cast<const T*>(h.data()), h.size(), reinterpret_cast<T*>(y.data()), y.size()));
+    }
+    void correlate(const std::vector<std::complex<T>>& x, const std::vector<std::complex<T>>& h, std::vector<std::complex<T>>& y,
+                   ConvMode mode = ConvMode::Full) const {
+        check_domain(true);
+        check(Api<T>::conv_host(raw_, PHASTFT_CONV_CORRELATE, static_cast<int>(mode), reinterpret_cast<const T*>(x.data()), x.size(),
+                                reinterpret_cast<const T*>(h.data()), h.size(), reinterpret_cast<T*>(y.data()), y.size()));
+    }
+    /// `batch` members on device pointers: x at b * x_stride, h at b * h_stride (0: one filter), y at b * y_stride, in values
+    /// (complex ones, as T pairs aligned to 2 * sizeof(T), for a complex plan)
+    void convolve_device(const T* d_x, std::size_t x_stride, const T* d_h, std::size_t h_stride, T* d_y, std::size_t y_stride,
+                         std::size_t batch, ConvMode mode = ConvMode::Full, void* stream = nullptr) const {
+        check(Api<T>::conv_dev(raw_, PHASTFT_CONV_CONVOLVE, static_cast<int>(mode), d_x, x_stride, d_h, h_stride, d_y, y_stride, batch, stream));
+    }
+    void correlate_device(const T* d_x, std::size_t x_stride, const T* d_h, std::size_t h_stride, T* d_y, std::size_t y_stride,
+                          std::size_t batch, ConvMode mode = ConvMode::Full, void* stream = nullptr) const {
+        check(Api<T>::conv_dev(raw_, PHASTFT_CONV_CORRELATE, static_cast<int>(mode), d_x, x_stride, d_h, h_stride, d_y, y_stride, batch, stream));
+    }
+  private:
+    // the host entry counts lengths in values of the planner's domain, so vectors of the other domain must not reach it
+    void check_domain(bool complex_operands) const {
+        if (complex_operands != cplx_)
+            throw Panic(PHASTFT_ERR_INVALID_ARG, std::string("PlannerConv domain mismatch: the planner was built for ") +
+                                                     (cplx_ ? "complex" : "real") + " operands, the vectors are " +
+                                                     (complex_operands ? "complex" : "real"));
+    }
+    typename Api<T>::Conv* raw_ = nullptr;
+    std::size_t n_x_ = 0, n_h_ = 0;
+    bool cplx_ = false;
+};
 }  // namespace detail
 
 using PlannerDit64 = detail::PlannerDit<double>;
@@ -354,6 +440,10 @@ using R2rKind = detail::R2rKind;
 using R2rNorm = detail::R2rNorm;
 using PlannerDct64 = detail::PlannerDct<double>;
 using PlannerDct32 = detail::PlannerDct<float>;
+using ConvMode = detail::ConvMode;
+using PlannerConv64 = detail::PlannerConv<double>;
+using PlannerConv32 = detail::PlannerConv<float>;
+using detail::conv_out_len;
 
 // ---- c2c (lib.rs:143-226, algorithms/dit.rs:263,338): in place on planar vectors -----------------------
 inline void fft_64_dit_with_planner_and_opts(std::vector<double>& reals, std::vector<double>& imags, Direction d, const PlannerDit64& p, const Options&) {

@@ -19,6 +19,9 @@ int main() {
     fails += !panics_with([] { PlannerDit32 p(0); }, "power of two");
     fails += !panics_with([] { PlannerR2c64 p(6); }, "n must be a power of 2 >= 4");
     fails += !panics_with([] { PlannerDct64 p(0); }, "n must be >= 1");
+    fails += !panics_with([] { PlannerConv64 p(0, 5); }, "n_x and n_h must be >= 1");
+    fails += !panics_with([] { PlannerConv32 p(std::size_t(1) << 30, 2, 0, true); }, "above 2^30");
+    fails += conv_out_len(10, 4, ConvMode::Full) != 13 || conv_out_len(10, 4, ConvMode::Same) != 10 || conv_out_len(4, 10, ConvMode::Valid) != 7;
     fails += !panics_with([] { std::vector<float> x(2), a(2), b(2); r2c_fft_f32(x, a, b); }, "n must be a power of 2 >= 4");
     Options o = Options::guess_options(1 << 16);
     fails += !(o.multithreaded_bit_reversal && o.smallest_parallel_chunk_size == 16384);
@@ -57,6 +60,32 @@ int main() {
         p.transform(R2rKind::Dct2, R2rNorm::Backward, x, y);
         p.transform(R2rKind::Dct3, R2rNorm::Forward, y, y);
         for (std::size_t i = 0; i < n; ++i) fails += std::fabs(y[i] - x[i]) > 1e-12;
+    }
+    {   // additive surface: convolution and correlation against direct sums, real and complex
+        const std::size_t nx = 300, nh = 37;
+        PlannerConv64 p(nx, nh);
+        fails += p.fft_len() != 512 || p.describe().find("n_x=300 n_h=37 f64 conv real L=2^9 | ") != 0;
+        std::vector<double> x(nx), h(nh), y(p.out_len(ConvMode::Valid));
+        for (std::size_t i = 0; i < nx; ++i) x[i] = std::sin(0.37 * i);
+        for (std::size_t i = 0; i < nh; ++i) h[i] = std::cos(0.21 * i);
+        p.convolve(x, h, y, ConvMode::Valid);
+        for (std::size_t j = 0; j < y.size(); ++j) {
+            double s = 0;
+            for (std::size_t k = 0; k < nh; ++k) s += x[j + nh - 1 - k] * h[k];
+            fails += std::fabs(y[j] - s) > 1e-12;
+        }
+        fails += !panics_with([&] { std::vector<std::complex<double>> a(nx), b(nh), c(nx); p.convolve(a, b, c, ConvMode::Same); }, "domain mismatch");
+        PlannerConv32 q(nx, nh, 0, true);
+        fails += !panics_with([&] { std::vector<float> a(nx), b(nh), c(nx + nh - 1); q.correlate(a, b, c); }, "domain mismatch");
+        std::vector<std::complex<float>> cx(nx), ch(nh), cy(q.out_len(ConvMode::Valid));
+        for (std::size_t i = 0; i < nx; ++i) cx[i] = {std::sin(0.37f * i), std::cos(0.5f * i)};
+        for (std::size_t i = 0; i < nh; ++i) ch[i] = {std::cos(0.21f * i), 0.25f};
+        q.correlate(cx, ch, cy, ConvMode::Valid);
+        for (std::size_t j = 0; j < cy.size(); ++j) {
+            std::complex<double> s = 0;
+            for (std::size_t k = 0; k < nh; ++k) s += std::complex<double>(cx[j + k]) * std::conj(std::complex<double>(ch[k]));
+            fails += std::abs(std::complex<double>(cy[j]) - s) > 1e-4;
+        }
     }
     std::printf("gpu checks: %d failures\n", fails);
     return fails;

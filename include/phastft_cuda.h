@@ -55,7 +55,8 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * last ODD pass only, in phastft_fft_interleaved_any_*: R, C and NT as in the planar call), R2C-UNTANGLE-IL / C2R-PRE-IL /
  * CHIRP-POST-R2C-IL / CHIRP-PRE-C2R-IL / SMOOTH-PRE-C2R-IL / ODD-R2C-IL / SMOOTH-POST-R2C-IL (the spectrum's end of
  * phastft_{r2c,c2r}_interleaved_any_*, whose halved mixed r2c's last pass is ODD-IL), DCT-PRE-<kind> / DCT-POST-<kind> (the ends of
- * phastft_dct_*, kind DCT2, DCT3, DST2 or DST3: R=<N>, C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * phastft_dct_*, kind DCT2, DCT3, DST2 or DST3: R=<N>, C=<members>), CONV-PRE / CONV-MUL / CONV-POST (phastft_conv_*: R=<L>,
+ * C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), c2r-in-il (the same from interleaved bins), cluster, pipe or pipe-tma; " pdl" marks
  * programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
@@ -498,6 +499,59 @@ PHASTFT_API int32_t phastft_dct_f64_host(const phastft_plan_dct_f64* plan, int k
                                          double* out, size_t len_out);
 PHASTFT_API int32_t phastft_dct_f32_host(const phastft_plan_dct_f32* plan, int kind, int norm, const float* in, size_t len_in,
                                          float* out, size_t len_out);
+
+/* ---- linear convolution and cross-correlation of real or complex signals of any lengths (scipy.signal) --------------------
+ * op PHASTFT_CONV_CONVOLVE: scipy.signal.fftconvolve(x, h, mode); PHASTFT_CONV_CORRELATE: scipy.signal.correlate(x, h, mode),
+ * i.e. convolution with conj(h reversed).  Windows of the full convolution y[j] = sum_k x[k] h[j - k], 0 <= j < n_x + n_h - 1:
+ *   PHASTFT_CONV_FULL   start 0,                    length n_x + n_h - 1
+ *   PHASTFT_CONV_SAME   start (n_h - 1) / 2,        length n_x
+ *   PHASTFT_CONV_VALID  start min(n_x, n_h) - 1,    length |n_x - n_h| + 1
+ * phastft_conv_out_len gives that length (0 for a bad mode or a zero length).
+ * _create: domain PHASTFT_CONV_REAL or PHASTFT_CONV_COMPLEX; the plan transforms at L = 2^ceil(log2(n_x + n_h - 1)), at least
+ * 4 (_fft_len), on the real any-length plan (interleaved r2c / c2r) or the complex one (interleaved forward / reverse).  n_x or
+ * n_h of 0, a bad domain, or L above 2^31 (real) / 2^30 (complex) return PHASTFT_ERR_INVALID_ARG before the device is touched.
+ * describe() is "n_x=<n_x> n_h=<n_h> <prec> conv <real|complex> L=2^<k> | " followed by the inner plan's describe().
+ * Each call runs CONV-PRE over the B signals and H filters (H = B, or 1 when h_stride == 0 or B == 1), the inner forward
+ * transform of those B + H members, CONV-MUL and the inverse on the B signals, and CONV-POST; the inverse's 1/L is the only
+ * scale.
+ * _dev: member b reads n_x values at d_x + b * x_stride and n_h at d_h + b * h_stride (h_stride 0: one filter for every member)
+ * and writes the window at d_y + b * y_stride.  Real values: any element offsets.  Complex values: interleaved (re, im) pairs,
+ * strides in complex values, pointers aligned to 2 * sizeof(T).  d_y may equal d_x or d_h.  With batch > 1, x_stride < n_x,
+ * y_stride < the output length, or h_stride neither 0 nor >= n_h; NULL or misaligned pointers; or a bad op or mode return
+ * PHASTFT_ERR_INVALID_ARG before any launch; batch == 0 does nothing.  The workspace follows the any-length plans' protocol:
+ * it grows outside a stream capture only (_reserve(batch) grows it and the inner plan's for `batch` pairwise members), and a
+ * call on another stream waits for the previous one.
+ * _host: synchronous, through a plan-owned staging buffer (allocated by the first host call); lengths in values (complex
+ * ones for the complex domain): len_x != n_x or len_h != n_h is PHASTFT_ERR_INPUT_LEN, len_y != the output length
+ * PHASTFT_ERR_OUTPUT_LEN. */
+#define PHASTFT_CONV_REAL 0
+#define PHASTFT_CONV_COMPLEX 1
+#define PHASTFT_CONV_CONVOLVE 0
+#define PHASTFT_CONV_CORRELATE 1
+#define PHASTFT_CONV_FULL 0
+#define PHASTFT_CONV_SAME 1
+#define PHASTFT_CONV_VALID 2
+typedef struct phastft_plan_conv_f64 phastft_plan_conv_f64;
+typedef struct phastft_plan_conv_f32 phastft_plan_conv_f32;
+PHASTFT_API size_t phastft_conv_out_len(size_t n_x, size_t n_h, int mode);
+PHASTFT_API int32_t phastft_plan_conv_f64_create(size_t n_x, size_t n_h, int domain, int device, phastft_plan_conv_f64** out);
+PHASTFT_API int32_t phastft_plan_conv_f32_create(size_t n_x, size_t n_h, int domain, int device, phastft_plan_conv_f32** out);
+PHASTFT_API void phastft_plan_conv_f64_destroy(phastft_plan_conv_f64* plan);
+PHASTFT_API void phastft_plan_conv_f32_destroy(phastft_plan_conv_f32* plan);
+PHASTFT_API size_t phastft_plan_conv_f64_fft_len(const phastft_plan_conv_f64* plan);
+PHASTFT_API size_t phastft_plan_conv_f32_fft_len(const phastft_plan_conv_f32* plan);
+PHASTFT_API const char* phastft_plan_conv_f64_describe(const phastft_plan_conv_f64* plan);
+PHASTFT_API const char* phastft_plan_conv_f32_describe(const phastft_plan_conv_f32* plan);
+PHASTFT_API int32_t phastft_plan_conv_f64_reserve(const phastft_plan_conv_f64* plan, size_t batch);
+PHASTFT_API int32_t phastft_plan_conv_f32_reserve(const phastft_plan_conv_f32* plan, size_t batch);
+PHASTFT_API int32_t phastft_conv_f64_dev(const phastft_plan_conv_f64* plan, int op, int mode, const double* d_x, size_t x_stride,
+                                         const double* d_h, size_t h_stride, double* d_y, size_t y_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_conv_f32_dev(const phastft_plan_conv_f32* plan, int op, int mode, const float* d_x, size_t x_stride,
+                                         const float* d_h, size_t h_stride, float* d_y, size_t y_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_conv_f64_host(const phastft_plan_conv_f64* plan, int op, int mode, const double* x, size_t len_x,
+                                          const double* h, size_t len_h, double* y, size_t len_y);
+PHASTFT_API int32_t phastft_conv_f32_host(const phastft_plan_conv_f32* plan, int op, int mode, const float* x, size_t len_x,
+                                          const float* h, size_t len_h, float* y, size_t len_y);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

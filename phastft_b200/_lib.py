@@ -138,6 +138,13 @@ SIGNATURES = {
     "phastft_plan_dct_{s}_reserve": ([_vp, _sz], _i32),
     "phastft_dct_{s}_dev": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
     "phastft_dct_{s}_host": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz], _i32),
+    "phastft_plan_conv_{s}_create": ([_sz, _sz, _ci, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_conv_{s}_destroy": ([_vp], None),
+    "phastft_plan_conv_{s}_fft_len": ([_vp], _sz),
+    "phastft_plan_conv_{s}_describe": ([_vp], C.c_char_p),
+    "phastft_plan_conv_{s}_reserve": ([_vp, _sz], _i32),
+    "phastft_conv_{s}_dev": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_conv_{s}_host": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
 }
 def check(code: int):
     if code != OK:
@@ -175,6 +182,15 @@ def any_mixed_factorization(n: int):
     return p.value, qa.value, qb.value
 
 
+lib.phastft_conv_out_len.argtypes = [_sz, _sz, _ci]
+lib.phastft_conv_out_len.restype = _sz
+
+
+def conv_out_len(n_x: int, n_h: int, mode: int) -> int:
+    """Host-only: the output length of a PHASTFT_CONV_* mode (0 for a bad mode or a zero length)."""
+    return int(lib.phastft_conv_out_len(int(n_x), int(n_h), int(mode)))
+
+
 lib.phastft_plan_tune_candidates.argtypes = [_sz, _ci, C.POINTER(_ci), C.POINTER(_ci), _ci, C.POINTER(_ci)]
 lib.phastft_plan_tune_candidates.restype = _i32
 
@@ -194,7 +210,7 @@ def plan_tune_candidates(n: int, precision_bits: int = 64):
 
 
 GLOBAL_SYMBOLS = ["phastft_host_register", "phastft_host_unregister", "phastft_oneshot_cache_clear", "phastft_plan_factorization",
-                  "phastft_plan_tune_candidates", "phastft_any_mixed_factorization", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
+                  "phastft_plan_tune_candidates", "phastft_any_mixed_factorization", "phastft_conv_out_len", "phastft_last_error", "phastft_version", "phastft_launch_count", "phastft_last_launches",
                   "phastft_last_scribble_bytes",
                   "phastft_device_count", "phastft_options_default", "phastft_options_guess"]
 

@@ -48,6 +48,7 @@ __all__ = [
     "r2c_interleaved_any_batch", "c2r_interleaved_any_batch",
     "PlannerDct64", "PlannerDct32", "dct_f64_with_planner", "dct_f32_with_planner", "dst_f64_with_planner", "dst_f32_with_planner",
     "dct_batch", "dst_batch",
+    "PlannerConv64", "PlannerConv32", "convolve_with_planner", "correlate_with_planner", "convolve_batch", "correlate_batch",
 ]
 
 
@@ -1168,3 +1169,174 @@ def dst_batch(x, out, planner, batch: int, type: int = 2, norm: str = "backward"
               out_stride: int | None = None) -> None:
     """dct_batch for the DST."""
     _r2r(True, x, out, planner, int(batch), type, norm, in_stride, out_stride)
+
+
+# ----------------------------------------------------------------------------------------------
+# linear convolution and cross-correlation of real or complex signals (scipy.signal.fftconvolve / correlate)
+# ----------------------------------------------------------------------------------------------
+_CONV_MODES = {"full": 0, "same": 1, "valid": 2}
+
+
+class _PlannerConv:
+    _sfx = ""
+    _dtype = None
+
+    def __init__(self, n_x: int, n_h: int, device: int = 0, complex: bool = False):
+        """Convolution and correlation of n_x values with n_h values (both >= 1), real or complex (interleaved complex128 /
+        complex64), over an L-point transform, L = 2^ceil(log2(n_x + n_h - 1)) but at least 4 (`fft_len`).  n_x or n_h of 0,
+        or L above 2^31 (real) / 2^30 (complex), raise PhastFTPanic(13) before the device is touched."""
+        self._h = C.c_void_p()
+        self.device = int(device)
+        self.complex = bool(complex)
+        check(fn("phastft_plan_conv_{s}_create", self._sfx)(int(n_x), int(n_h), int(self.complex), self.device, C.byref(self._h)))
+        self.n_x, self.n_h = int(n_x), int(n_h)
+
+    @property
+    def fft_len(self) -> int:
+        """L, the length of the transforms the plan runs."""
+        return int(fn("phastft_plan_conv_{s}_fft_len", self._sfx)(self._h))
+
+    def out_len(self, mode: str = "full") -> int:
+        """The output length of `mode`: n_x + n_h - 1 (full), n_x (same) or |n_x - n_h| + 1 (valid)."""
+        from ._lib import conv_out_len
+        return conv_out_len(self.n_x, self.n_h, _conv_mode(mode))
+
+    def describe(self) -> str:
+        """"n_x=<n_x> n_h=<n_h> <prec> conv <real|complex> L=2^<k> | " followed by the inner plan's describe()."""
+        return fn("phastft_plan_conv_{s}_describe", self._sfx)(self._h).decode()
+
+    def reserve(self, batch: int) -> None:
+        """Make every allocation a call of `batch` pairwise members would make now (otherwise the first larger call makes
+        them, synchronising the device -- an error inside a CUDA-graph capture)."""
+        check(fn("phastft_plan_conv_{s}_reserve", self._sfx)(self._h, int(batch)))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._h = None
+            try:
+                fn("phastft_plan_conv_{s}_destroy", self._sfx)(h)
+            except (AttributeError, TypeError):      # interpreter shutdown: the module globals are already gone
+                pass
+
+
+class PlannerConv64(_PlannerConv):
+    _sfx, _dtype = "f64", np.float64
+
+
+class PlannerConv32(_PlannerConv):
+    _sfx, _dtype = "f32", np.float32
+
+
+def _conv_mode(mode) -> int:
+    if not isinstance(mode, str) or mode not in _CONV_MODES:
+        raise ValueError(f"mode must be 'full', 'same' or 'valid', got {mode!r}")
+    return _CONV_MODES[mode]
+
+
+def _conv_operand(planner, a, what: str, on_device: bool):
+    """`a` checked against the planner: a contiguous 1-D torch CUDA tensor (on_device) or numpy array of its dtype (float64 /
+    float32, or complex128 / complex64 for a complex planner).  A wrong dtype raises ValueError, a wrong kind TypeError."""
+    cplx = planner.complex
+    if on_device:
+        import torch
+        if not _is_torch(a) or not a.is_cuda:
+            raise TypeError(f"{what}: pass every operand as a torch CUDA tensor, or every one as a numpy array")
+        want = {("f64", False): torch.float64, ("f32", False): torch.float32,
+                ("f64", True): torch.complex128, ("f32", True): torch.complex64}[(planner._sfx, cplx)]
+        if a.dtype != want:
+            raise ValueError(f"{what}: expected dtype {want} for this planner, got {a.dtype}")
+        if a.dim() != 1 or not a.is_contiguous():
+            raise ValueError(f"{what}: expected a contiguous 1-D tensor")
+        return a
+    if not isinstance(a, np.ndarray):
+        raise TypeError(f"{what}: pass every operand as a torch CUDA tensor, or every one as a numpy array")
+    want = np.dtype({("f64", False): np.float64, ("f32", False): np.float32,
+                     ("f64", True): np.complex128, ("f32", True): np.complex64}[(planner._sfx, cplx)])
+    if a.dtype != want:
+        raise ValueError(f"{what}: expected dtype {want} for this planner, got {a.dtype}")
+    if a.ndim != 1 or not a.flags.c_contiguous:
+        raise ValueError(f"{what}: expected a contiguous 1-D array")
+    return a
+
+
+def _conv_dev(op, x, h, out, planner, batch, mode, x_stride, h_stride, out_stride):
+    """One device call on torch tensors; a complex operand whose pointer is not pair-aligned goes through an aligned copy."""
+    def aligned(t):
+        return not planner.complex or _pair_aligned(t)
+    xs = x if aligned(x) else x.clone()
+    hs = h if aligned(h) else h.clone()
+    work = out if aligned(out) else out.clone()   # the clone keeps what lies between members
+    check(fn("phastft_conv_{s}_dev", planner._sfx)(planner._h, op, mode, C.c_void_p(xs.data_ptr()), x_stride,
+                                                   C.c_void_p(hs.data_ptr()), h_stride, C.c_void_p(work.data_ptr()), out_stride,
+                                                   int(batch), _torch_stream(out)))
+    if work is not out:
+        out.copy_(work)
+
+
+def _conv_with_planner(op, x, h, out, planner, mode):
+    m = _conv_mode(mode)
+    if not isinstance(planner, _PlannerConv):
+        raise TypeError("expected a PlannerConv64 or PlannerConv32")
+    on_device = _is_torch(out)
+    x = _conv_operand(planner, x, "x", on_device)
+    h = _conv_operand(planner, h, "h", on_device)
+    out = _conv_operand(planner, out, "out", on_device)
+    n_y = planner.out_len(mode)
+    for what, a, n in (("x", x, planner.n_x), ("h", h, planner.n_h), ("out", out, n_y)):
+        have = a.numel() if on_device else a.size
+        if have != n:
+            raise ValueError(f"{what} has {have} values, the planner expects {n}")
+    if on_device:
+        _conv_dev(op, x, h, out, planner, 1, m, planner.n_x, planner.n_h, n_y)
+        return
+    if not out.flags.writeable:
+        raise ValueError("out is read-only")
+    check(fn("phastft_conv_{s}_host", planner._sfx)(planner._h, op, m, x.ctypes.data_as(C.c_void_p), x.size,
+                                                    h.ctypes.data_as(C.c_void_p), h.size, out.ctypes.data_as(C.c_void_p), out.size))
+
+
+def _conv_batch(op, x, h, out, planner, batch, mode, x_stride, h_stride, out_stride):
+    m = _conv_mode(mode)
+    if not isinstance(planner, _PlannerConv):
+        raise TypeError("expected a PlannerConv64 or PlannerConv32")
+    x = _conv_operand(planner, x, "x", True)
+    h = _conv_operand(planner, h, "h", True)
+    out = _conv_operand(planner, out, "out", True)
+    batch = int(batch)
+    if batch < 0:
+        raise ValueError("batch < 0")
+    n_y = planner.out_len(mode)
+    x_stride = planner.n_x if x_stride is None else int(x_stride)
+    h_stride = planner.n_h if h_stride is None else int(h_stride)
+    out_stride = n_y if out_stride is None else int(out_stride)
+    for what, a, stride, n in (("x", x, x_stride, planner.n_x), ("h", h, h_stride, planner.n_h), ("out", out, out_stride, n_y)):
+        if batch and a.numel() < (batch - 1) * stride + n:
+            raise ValueError(f"{what} has {a.numel()} values, fewer than (batch - 1) * stride + {n}")
+    _conv_dev(op, x, h, out, planner, batch, m, x_stride, h_stride, out_stride)
+
+
+def convolve_with_planner(x, h, out, planner, mode: str = "full") -> None:
+    """scipy.signal.fftconvolve(x, h, mode) into out: numpy arrays (synchronous) or 1-D torch CUDA tensors (torch's current
+    stream) of the planner's dtype, with len(x) == planner.n_x, len(h) == planner.n_h and len(out) == planner.out_len(mode).
+    out may be x or h (when the lengths allow)."""
+    _conv_with_planner(0, x, h, out, planner, mode)
+
+
+def correlate_with_planner(x, h, out, planner, mode: str = "full") -> None:
+    """scipy.signal.correlate(x, h, mode) into out: convolve_with_planner with conj(h reversed)."""
+    _conv_with_planner(1, x, h, out, planner, mode)
+
+
+def convolve_batch(x, h, out, planner, batch: int, mode: str = "full", x_stride: int | None = None, h_stride: int | None = None,
+                   out_stride: int | None = None) -> None:
+    """`batch` convolutions on flat 1-D torch CUDA tensors: member b convolves x[b * x_stride:][:n_x] with h[b * h_stride:][:n_h]
+    (h_stride 0: one filter for every member) into out[b * out_stride:][:out_len(mode)].  Defaults: n_x, n_h, out_len(mode);
+    strides in values (complex ones for a complex planner)."""
+    _conv_batch(0, x, h, out, planner, batch, mode, x_stride, h_stride, out_stride)
+
+
+def correlate_batch(x, h, out, planner, batch: int, mode: str = "full", x_stride: int | None = None, h_stride: int | None = None,
+                    out_stride: int | None = None) -> None:
+    """convolve_batch for scipy.signal.correlate."""
+    _conv_batch(1, x, h, out, planner, batch, mode, x_stride, h_stride, out_stride)

@@ -1661,4 +1661,67 @@ __global__ void __launch_bounds__(256) dct_post_kernel(const __grid_constant__ D
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// CONV-PRE / CONV-MUL / CONV-POST: the three elementwise kernels of linear convolution and correlation over an L-point
+// transform (L a power of two >= n_x + n_h - 1, so the circular convolution at L is the linear one).  Workspace members are
+// L apart in the signal region (reals or complex values) and `spec_stride` bins apart in the spectrum region (the same memory
+// for complex signals).  PRE pads member m < n_xm (x) or m - n_xm (h; reversed and conjugated for correlation) to L; MUL forms
+// X_b H_b in place over `bins` bins, or X_b H_0 when h_bcast; POST copies the window [start, start + out_len) of member b to
+// the caller.  The caller's arrays (any stride and offset, complex ones as pairs aligned to 2 * sizeof(T)) are accessed one
+// element at a time.  A member-major grid of 256-thread blocks, member m0 + blockIdx.x / blocks_per_member.
+template <typename T>
+struct ConvParams {
+    const T* x;                    // the caller's signals (PRE)
+    const T* h;                    // the caller's filters (PRE)
+    T* y;                          // the caller's output (POST)
+    T* sig;                        // the workspace signal region: member m at sig + m * L values
+    cx<T>* spec;                   // the workspace spectra: member m at spec + m * spec_stride
+    long long n_x, n_h, L, x_stride, h_stride, y_stride;   // strides in values (complex ones for complex signals)
+    long long n_xm;                // PRE: members below it are signals, the rest filters
+    long long start, out_len;      // POST's window
+    long long spec_stride, bins;   // MUL
+    long long m0;                  // the first member of this launch
+    int h_bcast;                   // MUL: one filter spectrum for every member
+    unsigned blocks_per_member;
+};
+
+template <typename T, bool CPLX>
+using conv_value_t = typename std::conditional<CPLX, cx<T>, T>::type;
+
+template <typename T, bool CPLX, bool CORR>
+__global__ void __launch_bounds__(256) conv_pre_kernel(const __grid_constant__ ConvParams<T> p) {
+    using E = conv_value_t<T, CPLX>;
+    const long long m = p.m0 + blockIdx.x / p.blocks_per_member;
+    const long long j = (long long)(blockIdx.x % p.blocks_per_member) * 256 + threadIdx.x;
+    if (j >= p.L) return;
+    E v;
+    if constexpr (CPLX) v = make_cx<T>(T(0), T(0)); else v = T(0);
+    if (m < p.n_xm) {
+        if (j < p.n_x) v = reinterpret_cast<const E*>(p.x)[m * p.x_stride + j];
+    } else if (j < p.n_h) {
+        v = reinterpret_cast<const E*>(p.h)[(m - p.n_xm) * p.h_stride + (CORR ? p.n_h - 1 - j : j)];
+        if constexpr (CPLX && CORR) v.y = -v.y;
+    }
+    reinterpret_cast<E*>(p.sig)[m * p.L + j] = v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) conv_mul_kernel(const __grid_constant__ ConvParams<T> p) {
+    const long long b = p.m0 + blockIdx.x / p.blocks_per_member;
+    const long long k = (long long)(blockIdx.x % p.blocks_per_member) * 256 + threadIdx.x;
+    if (k >= p.bins) return;
+    cx<T>* xb = p.spec + b * p.spec_stride + k;
+    const cx<T> hb = p.spec[(p.n_xm + (p.h_bcast ? 0 : b)) * p.spec_stride + k];
+    *xb = cmul<T>(*xb, hb);
+}
+
+template <typename T, bool CPLX>
+__global__ void __launch_bounds__(256) conv_post_kernel(const __grid_constant__ ConvParams<T> p) {
+    using E = conv_value_t<T, CPLX>;
+    const long long b = p.m0 + blockIdx.x / p.blocks_per_member;
+    const long long j = (long long)(blockIdx.x % p.blocks_per_member) * 256 + threadIdx.x;
+    if (j >= p.out_len) return;
+    reinterpret_cast<E*>(p.y)[b * p.y_stride + j] = reinterpret_cast<const E*>(p.sig)[b * p.L + p.start + j];
+}
+
 }  // namespace phast

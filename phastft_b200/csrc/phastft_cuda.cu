@@ -3721,6 +3721,206 @@ int32_t dct_host(const PlanDct<T>* pl, int kind, int norm, const T* in, size_t l
     return PHASTFT_OK;
 }
 
+// =================================================================================================
+// linear convolution and correlation of real or complex signals of any lengths: CONV-PRE, the L-point real plan's interleaved
+// r2c (or the complex plan's forward transform) on x and h together, CONV-MUL, the c2r (or reverse transform) on x, CONV-POST
+// (fft_kernels.cuh).  L = 2^ceil(log2(n_x + n_h - 1)), at least 4, so the circular convolution at L is the linear one.
+// =================================================================================================
+// The window of the full convolution (n_x + n_h - 1 values) that each PHASTFT_CONV_* mode returns, scipy.signal's; length 0
+// for a bad mode or an empty operand.
+size_t conv_out_len(size_t n_x, size_t n_h, int mode) {
+    if (n_x == 0 || n_h == 0) return 0;
+    switch (mode) {
+        case PHASTFT_CONV_FULL: return n_x + n_h - 1;
+        case PHASTFT_CONV_SAME: return n_x;
+        case PHASTFT_CONV_VALID: return std::max(n_x, n_h) - std::min(n_x, n_h) + 1;
+        default: return 0;
+    }
+}
+size_t conv_start(size_t n_x, size_t n_h, int mode) {
+    return mode == PHASTFT_CONV_SAME ? (n_h - 1) / 2 : mode == PHASTFT_CONV_VALID ? std::min(n_x, n_h) - 1 : 0;
+}
+
+template <typename T>
+struct PlanConv {
+    size_t n_x = 0, n_h = 0, L = 0;
+    int device = 0;
+    bool cplx = false;
+    PlanR2cAny<T>* real = nullptr;     // real signals: the L-point real plan (its power-of-two r2c plan)
+    PlanAny<T>* cinner = nullptr;      // complex signals: the L-point complex plan
+    // per call of C = B + H members (B signals, H = B filters or one broadcast): real, C x L reals then C x (L/2 + 1) bins;
+    // complex, C x L values transformed in place.  The AnyWorkspace protocol.
+    mutable AnyWorkspace<T> w;
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then w.mu, then the inner plan's)
+    mutable T* stage = nullptr;        // host-API staging: x, h and y back to back; allocated by the first host call
+    std::string description;
+    size_t member_elems() const { return cplx ? L : L + 1; }        // complex values
+    size_t stage_elems() const { return n_x + n_h + conv_out_len(n_x, n_h, PHASTFT_CONV_FULL); }   // values (T or complex)
+    cudaStream_t host_stream() const { return cplx ? cinner->pow2->stream : real->pow2->inner->stream; }
+    ~PlanConv() {
+        DeviceGuard g(device);
+        w.destroy();
+        if (stage) cudaFree(stage);
+        delete real;
+        delete cinner;
+    }
+};
+
+template <typename T>
+int32_t build_plan_conv(size_t n_x, size_t n_h, int domain, int device, PlanConv<T>** out) {
+    if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
+    *out = nullptr;
+    if (n_x == 0 || n_h == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n_x and n_h must be >= 1");
+    if (domain != PHASTFT_CONV_REAL && domain != PHASTFT_CONV_COMPLEX)
+        return fail(PHASTFT_ERR_INVALID_ARG, "domain must be PHASTFT_CONV_REAL or PHASTFT_CONV_COMPLEX");
+    const bool cplx = domain == PHASTFT_CONV_COMPLEX;
+    const int lmax = cplx ? 30 : 31;       // the largest complex plan, the largest real one
+    const size_t top = size_t(1) << lmax;
+    if (n_x > top || n_h > top || n_x + n_h - 1 > top)
+        return fail(PHASTFT_ERR_INVALID_ARG, "n_x + n_h - 1 = " + std::to_string(n_x + n_h - 1) + " is above 2^" + std::to_string(lmax) +
+                                             " (the largest " + (cplx ? "complex" : "real") + " transform length L)");
+    int ll = 2;
+    while ((size_t(1) << ll) < n_x + n_h - 1) ++ll;
+    std::unique_ptr<PlanConv<T>> pl(new PlanConv<T>());
+    pl->n_x = n_x; pl->n_h = n_h; pl->L = size_t(1) << ll; pl->device = device; pl->cplx = cplx;
+    if (int32_t st = cplx ? build_plan_any<T>(pl->L, device, PHASTFT_ANY_AUTO, &pl->cinner)
+                          : build_plan_r2c_any<T>(pl->L, device, PHASTFT_ANY_AUTO, &pl->real))
+        return st;
+    DeviceGuard g(device);
+    if (int32_t st = pl->w.init(2 * pl->member_elems())) return st;   // room for one lone call; batched calls grow it
+    pl->description = "n_x=" + std::to_string(n_x) + " n_h=" + std::to_string(n_h) + (sizeof(T) == 8 ? " f64" : " f32") + " conv " +
+                      (cplx ? "complex" : "real") + " L=2^" + std::to_string(ll) + " | ";
+    *out = pl.release();
+    return PHASTFT_OK;
+}
+
+template <typename T>
+std::string conv_description(const PlanConv<T>* pl) {
+    return pl->description + (pl->cplx ? pl->cinner->description : r2c_any_description(pl->real));
+}
+
+// Every allocation a call of `batch` pairwise members would make: the inner plan's for the forward call of 2 x batch members
+// and the inverse of batch, and the workspace.
+template <typename T>
+int32_t conv_reserve(const PlanConv<T>* pl, size_t batch) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    for (size_t b : {2 * batch, batch})
+        if (int32_t st = pl->cplx ? any_reserve(pl->cinner, b) : r2c_any_reserve(pl->real, b)) return st;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    return pl->w.grow(2 * batch * pl->member_elems(), 2 * batch);
+}
+
+// One CONV-PRE, CONV-MUL or CONV-POST over `members` members from member 0, `threads` threads each, in launches of at most
+// 2^31 - 1 blocks.  Launch record: R = L, C = the members of that launch.
+template <typename T>
+int32_t launch_conv_stage(int stage, bool cplx, bool corr, ConvParams<T> p, size_t threads, size_t members, cudaStream_t stream) {
+    static const char* const names[3] = {"CONV-PRE", "CONV-MUL", "CONV-POST"};
+    const size_t bpm = (threads + 255) / 256;
+    p.blocks_per_member = (unsigned)bpm;
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    for (size_t done = 0; done < members; done += max_members) {
+        const size_t nb = std::min(members - done, max_members);
+        p.m0 = (long long)done;
+        launch_conv<T>(stage, cplx, corr, p, (unsigned)(nb * bpm), stream);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({names[stage], (int)std::min<long long>(p.L, INT32_MAX), 0, (int)nb, 256, 0, "plain", false});
+    }
+    return PHASTFT_OK;
+}
+
+// Member b convolves (op PHASTFT_CONV_CONVOLVE) or correlates the n_x values at d_x + b * x_stride with the n_h values at
+// d_h + b * h_stride (h_stride 0: one filter for every member) and writes the mode's window at d_y + b * y_stride.  Values are
+// reals, or complex (re, im) pairs with strides in complex values and pointers aligned to 2 * sizeof(T).  Any element offsets;
+// d_y may be d_x or d_h (CONV-PRE reads every input before CONV-POST writes).
+template <typename T>
+int32_t conv_dev(const PlanConv<T>* pl, int op, int mode, const T* d_x, size_t x_stride, const T* d_h, size_t h_stride, T* d_y,
+                 size_t y_stride, size_t batch, cudaStream_t stream) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (op != PHASTFT_CONV_CONVOLVE && op != PHASTFT_CONV_CORRELATE)
+        return fail(PHASTFT_ERR_INVALID_ARG, "op must be PHASTFT_CONV_CONVOLVE or PHASTFT_CONV_CORRELATE");
+    if (mode != PHASTFT_CONV_FULL && mode != PHASTFT_CONV_SAME && mode != PHASTFT_CONV_VALID)
+        return fail(PHASTFT_ERR_INVALID_ARG, "mode must be PHASTFT_CONV_FULL, _SAME or _VALID");
+    if (!d_x) return fail(PHASTFT_ERR_INVALID_ARG, "d_x == NULL");
+    if (!d_h) return fail(PHASTFT_ERR_INVALID_ARG, "d_h == NULL");
+    if (!d_y) return fail(PHASTFT_ERR_INVALID_ARG, "d_y == NULL");
+    const size_t n_x = pl->n_x, n_h = pl->n_h, L = pl->L, out_len = conv_out_len(n_x, n_h, mode);
+    if (batch > 1) {
+        if (x_stride < n_x) return fail(PHASTFT_ERR_INVALID_ARG, "x_stride must be >= n_x = " + std::to_string(n_x) + " (got " + std::to_string(x_stride) + ")");
+        if (h_stride != 0 && h_stride < n_h)
+            return fail(PHASTFT_ERR_INVALID_ARG, "h_stride must be 0 (one filter) or >= n_h = " + std::to_string(n_h) + " (got " + std::to_string(h_stride) + ")");
+        if (y_stride < out_len)
+            return fail(PHASTFT_ERR_INVALID_ARG, "y_stride must be >= the output length " + std::to_string(out_len) + " (got " + std::to_string(y_stride) + ")");
+    }
+    if (pl->cplx) {
+        if (int32_t st = check_pair_alignment(d_x, "d_x")) return st;
+        if (int32_t st = check_pair_alignment(d_h, "d_h")) return st;
+        if (int32_t st = check_pair_alignment(d_y, "d_y")) return st;
+    }
+    if (batch == 0) return PHASTFT_OK;
+    const size_t nh_members = batch == 1 || h_stride == 0 ? 1 : batch, members = batch + nh_members;
+    const size_t bins = pl->cplx ? L : L / 2 + 1;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    bool capturing = false;
+    if (int32_t st = pl->w.acquire(members * pl->member_elems(), members, stream, "phastft_plan_conv_*_reserve", capturing)) return st;
+    T* sig = reinterpret_cast<T*>(pl->w.ws);
+    cx<T>* spec = pl->cplx ? pl->w.ws : pl->w.ws + members * L / 2;
+    ConvParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.x = d_x; p.h = d_h; p.y = d_y; p.sig = sig; p.spec = spec;
+    p.n_x = (long long)n_x; p.n_h = (long long)n_h; p.L = (long long)L;
+    p.x_stride = (long long)x_stride; p.h_stride = (long long)h_stride; p.y_stride = (long long)y_stride;
+    p.n_xm = (long long)batch;
+    p.start = (long long)conv_start(n_x, n_h, mode); p.out_len = (long long)out_len;
+    p.spec_stride = (long long)bins; p.bins = (long long)bins;
+    p.h_bcast = nh_members == 1;
+    const bool cplx = pl->cplx, corr = op == PHASTFT_CONV_CORRELATE;
+    int32_t st = launch_conv_stage<T>(CONV_STAGE_PRE, cplx, corr, p, L, members, stream);
+    if (!st) st = cplx ? any_interleaved_dev(pl->cinner, sig, PHASTFT_FORWARD, members, L, stream)
+                       : r2c_il_any_dev(pl->real, sig, L, reinterpret_cast<T*>(spec), bins, members, stream);
+    if (!st) st = launch_conv_stage<T>(CONV_STAGE_MUL, cplx, corr, p, bins, batch, stream);
+    if (!st) st = cplx ? any_interleaved_dev(pl->cinner, sig, PHASTFT_REVERSE, batch, L, stream)
+                       : c2r_il_any_dev(pl->real, reinterpret_cast<const T*>(spec), bins, sig, L, batch, stream);
+    if (!st) st = launch_conv_stage<T>(CONV_STAGE_POST, cplx, corr, p, out_len, batch, stream);
+    const int32_t rel = pl->w.release(stream, capturing);   // also after a failed launch: the kernels queued so far used it
+    return st ? st : rel;
+}
+
+// host slices, synchronous: x, h and y staged through one plan-owned buffer.  Lengths in values (complex ones for complex
+// signals): len_x != n_x or len_h != n_h is PHASTFT_ERR_INPUT_LEN, len_y != the mode's output length PHASTFT_ERR_OUTPUT_LEN.
+template <typename T>
+int32_t conv_host(const PlanConv<T>* pl, int op, int mode, const T* x, size_t len_x, const T* h, size_t len_h, T* y, size_t len_y) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    if (op != PHASTFT_CONV_CONVOLVE && op != PHASTFT_CONV_CORRELATE)
+        return fail(PHASTFT_ERR_INVALID_ARG, "op must be PHASTFT_CONV_CONVOLVE or PHASTFT_CONV_CORRELATE");
+    if (mode != PHASTFT_CONV_FULL && mode != PHASTFT_CONV_SAME && mode != PHASTFT_CONV_VALID)
+        return fail(PHASTFT_ERR_INVALID_ARG, "mode must be PHASTFT_CONV_FULL, _SAME or _VALID");
+    const size_t n_x = pl->n_x, n_h = pl->n_h, out_len = conv_out_len(n_x, n_h, mode);
+    if (len_x != n_x) return fail(PHASTFT_ERR_INPUT_LEN, "len_x " + std::to_string(len_x) + ", plan n_x = " + std::to_string(n_x));
+    if (len_h != n_h) return fail(PHASTFT_ERR_INPUT_LEN, "len_h " + std::to_string(len_h) + ", plan n_h = " + std::to_string(n_h));
+    if (len_y != out_len) return fail(PHASTFT_ERR_OUTPUT_LEN, "len_y " + std::to_string(len_y) + ", output length " + std::to_string(out_len));
+    if (!x || !h || !y) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    const size_t v = pl->cplx ? 2 : 1;        // T per value
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->host_stream();
+    {
+        std::lock_guard<std::mutex> lock(pl->w.mu);   // released before the device call, which takes it
+        if (!pl->stage) CUDA_TRY(cudaMalloc(&pl->stage, pl->stage_elems() * v * sizeof(T)));
+    }
+    T* sx = pl->stage;
+    T* sh = sx + n_x * v;
+    T* sy = sh + n_h * v;
+    CUDA_TRY(scribble(pl->w.scribble_on, pl->stage, pl->stage_elems() * v * sizeof(T), s));
+    CUDA_TRY(cudaMemcpyAsync(sx, x, n_x * v * sizeof(T), cudaMemcpyHostToDevice, s));
+    CUDA_TRY(cudaMemcpyAsync(sh, h, n_h * v * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = conv_dev(pl, op, mode, sx, n_x, sh, n_h, sy, out_len, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(y, sy, out_len * v * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -3736,6 +3936,8 @@ int32_t dct_host(const PlanDct<T>* pl, int kind, int norm, const T* in, size_t l
 #define AS_CR2CANY(T, p) reinterpret_cast<const PlanR2cAny<T>*>(p)
 #define AS_DCT(T, p) reinterpret_cast<PlanDct<T>*>(p)
 #define AS_CDCT(T, p) reinterpret_cast<const PlanDct<T>*>(p)
+#define AS_CONV(T, p) reinterpret_cast<PlanConv<T>*>(p)
+#define AS_CCONV(T, p) reinterpret_cast<const PlanConv<T>*>(p)
 
 extern "C" {
 
@@ -4091,9 +4293,39 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                      T* out, size_t lout) {                                                             \
         launches_reset();                                                                                               \
         return dct_host<T>(AS_CDCT(T, p), kind, norm, in, lin, out, lout);                                              \
+    }                                                                                                                   \
+    int32_t phastft_plan_conv_##SFX##_create(size_t n_x, size_t n_h, int domain, int device,                            \
+                                             phastft_plan_conv_##SFX** out) {                                           \
+        PlanConv<T>* pl = nullptr;                                                                                      \
+        int32_t st = build_plan_conv<T>(n_x, n_h, domain, device, &pl);                                                 \
+        if (out) *out = reinterpret_cast<phastft_plan_conv_##SFX*>(pl);                                                 \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    void phastft_plan_conv_##SFX##_destroy(phastft_plan_conv_##SFX* p) { delete AS_CONV(T, p); }                        \
+    size_t phastft_plan_conv_##SFX##_fft_len(const phastft_plan_conv_##SFX* p) { return p ? AS_CCONV(T, p)->L : 0; }    \
+    const char* phastft_plan_conv_##SFX##_describe(const phastft_plan_conv_##SFX* p) {                                  \
+        if (!p) return "";                                                                                              \
+        g_r2c_desc_text = conv_description<T>(AS_CCONV(T, p));                                                          \
+        return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
+    int32_t phastft_plan_conv_##SFX##_reserve(const phastft_plan_conv_##SFX* p, size_t batch) {                         \
+        return conv_reserve<T>(AS_CCONV(T, p), batch);                                                                  \
+    }                                                                                                                   \
+    int32_t phastft_conv_##SFX##_dev(const phastft_plan_conv_##SFX* p, int op, int mode, const T* x, size_t x_stride,   \
+                                     const T* h, size_t h_stride, T* y, size_t y_stride, size_t batch, void* s) {       \
+        launches_reset();                                                                                               \
+        return conv_dev<T>(AS_CCONV(T, p), op, mode, x, x_stride, h, h_stride, y, y_stride, batch, (cudaStream_t)s);    \
+    }                                                                                                                   \
+    int32_t phastft_conv_##SFX##_host(const phastft_plan_conv_##SFX* p, int op, int mode, const T* x, size_t len_x,     \
+                                      const T* h, size_t len_h, T* y, size_t len_y) {                                   \
+        launches_reset();                                                                                               \
+        return conv_host<T>(AS_CCONV(T, p), op, mode, x, len_x, h, len_h, y, len_y);                                    \
     }
 
 DEFINE_DIT_API(double, f64)
 DEFINE_DIT_API(float, f32)
+
+size_t phastft_conv_out_len(size_t n_x, size_t n_h, int mode) { return conv_out_len(n_x, n_h, mode); }
 
 }  // extern "C"

@@ -137,4 +137,9 @@ template <typename T> void launch_smooth_post_r2c_il(const SmoothPostParams<T>& 
 // defined in r2r.cu: DCT-PRE (`post` false) or DCT-POST of DctKind `kind`
 template <typename T> void launch_dct(bool post, int kind, const DctParams<T>& p, unsigned grid, cudaStream_t stream);
 
+// defined in conv.cu: CONV-PRE, CONV-MUL or CONV-POST (`stage`) for real or complex (`cplx`) signals, PRE for convolution or
+// correlation (`corr`)
+enum ConvStage { CONV_STAGE_PRE = 0, CONV_STAGE_MUL = 1, CONV_STAGE_POST = 2 };
+template <typename T> void launch_conv(int stage, bool cplx, bool corr, const ConvParams<T>& p, unsigned grid, cudaStream_t stream);
+
 }  // namespace phast

@@ -20,8 +20,8 @@ pub mod options;
 pub mod planner;
 
 use options::Options;
-use planner::{Direction, PlannerAny32, PlannerAny64, PlannerDit32, PlannerDit64, PlannerDct32, PlannerDct64, PlannerR2c32, PlannerR2c64, PlannerR2cAny32,
-              PlannerR2cAny64};
+use planner::{Direction, PlannerAny32, PlannerAny64, PlannerConv32, PlannerConv64, PlannerDit32, PlannerDit64, PlannerDct32, PlannerDct64,
+              PlannerR2c32, PlannerR2c64, PlannerR2cAny32, PlannerR2cAny64};
 
 /// Reference panic texts by status code (include/phastft_status.h).
 #[track_caller]
@@ -326,6 +326,71 @@ impl_dct!(dct_f64_with_planner, dct_f64_device_batch, f64, PlannerDct64, phastft
 impl_dct!(dct_f32_with_planner, dct_f32_device_batch, f32, PlannerDct32, phastft_dct_f32_host, phastft_dct_f32_dev);
 
 // ------------------------------------------------------------------------------------------------
+// Additive: linear convolution and cross-correlation (scipy.signal.fftconvolve / correlate)
+// ------------------------------------------------------------------------------------------------
+/// The output window of `PlannerConv*`: the whole linear convolution (n_x + n_h - 1 values), its centre n_x values from
+/// (n_h - 1) / 2, or the |n_x - n_h| + 1 values that need no zero padding, from min(n_x, n_h) - 1.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum ConvMode {
+    Full = 0,
+    Same = 1,
+    Valid = 2,
+}
+const CONV_CONVOLVE: i32 = 0;
+const CONV_CORRELATE: i32 = 1;
+/// The safe host functions pass slice lengths in values of the slice's element type, and the library reads and writes as many
+/// values of the planner's domain: a real slice given to a complex planner would be overrun, a complex one given to a real
+/// planner misread.  So they panic on a domain mismatch before any call.
+#[track_caller]
+fn check_conv_domain(planner_complex: bool, slices_complex: bool) {
+    if planner_complex != slices_complex {
+        panic!("PlannerConv domain mismatch: the planner was built for {} operands, the slices are {}",
+               if planner_complex { "complex" } else { "real" }, if slices_complex { "complex" } else { "real" });
+    }
+}
+macro_rules! impl_conv {
+    ($conv:ident, $corr:ident, $conv_dev:ident, $corr_dev:ident, $t:ty, $planner:ident, $ffi_host:ident, $ffi_dev:ident) => {
+        /// Real operands of a real planner: `y` gets the window of `mode` of x * h.  Panics on a length mismatch, and when
+        /// the planner was built for complex operands.
+        pub fn $conv(x: &[$t], h: &[$t], y: &mut [$t], mode: ConvMode, planner: &$planner) {
+            check_conv_domain(planner.is_complex(), false);
+            check(unsafe { ffi::$ffi_host(planner.raw, CONV_CONVOLVE, mode as i32, x.as_ptr(), x.len(), h.as_ptr(), h.len(),
+                                          y.as_mut_ptr(), y.len()) });
+        }
+        /// The cross-correlation of x with h (convolution with h reversed), as the convolution, with its panics.
+        pub fn $corr(x: &[$t], h: &[$t], y: &mut [$t], mode: ConvMode, planner: &$planner) {
+            check_conv_domain(planner.is_complex(), false);
+            check(unsafe { ffi::$ffi_host(planner.raw, CONV_CORRELATE, mode as i32, x.as_ptr(), x.len(), h.as_ptr(), h.len(),
+                                          y.as_mut_ptr(), y.len()) });
+        }
+        /// `batch` convolutions on device data: member b reads x at `d_x + b * x_stride`, h at `d_h + b * h_stride`
+        /// (`h_stride == 0`: one filter for every member) and writes the window at `d_y + b * y_stride`, stream-ordered.
+        /// Strides count values (complex ones, as `$t` pairs aligned to their size, for a complex planner).
+        ///
+        /// # Safety
+        /// The pointers must be device pointers valid for the members on the planner's device, counted in values of the
+        /// planner's domain (two `$t` per value for a complex planner).
+        pub unsafe fn $conv_dev(d_x: *const $t, x_stride: usize, d_h: *const $t, h_stride: usize, d_y: *mut $t, y_stride: usize,
+                                mode: ConvMode, planner: &$planner, batch: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$ffi_dev(planner.raw, CONV_CONVOLVE, mode as i32, d_x, x_stride, d_h, h_stride, d_y, y_stride, batch, stream));
+        }
+        /// The cross-correlation form of the device batch.
+        ///
+        /// # Safety
+        /// As for the convolution.
+        pub unsafe fn $corr_dev(d_x: *const $t, x_stride: usize, d_h: *const $t, h_stride: usize, d_y: *mut $t, y_stride: usize,
+                                mode: ConvMode, planner: &$planner, batch: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$ffi_dev(planner.raw, CONV_CORRELATE, mode as i32, d_x, x_stride, d_h, h_stride, d_y, y_stride, batch, stream));
+        }
+    };
+}
+impl_conv!(convolve_f64_with_planner, correlate_f64_with_planner, convolve_f64_device_batch, correlate_f64_device_batch, f64,
+           PlannerConv64, phastft_conv_f64_host, phastft_conv_f64_dev);
+impl_conv!(convolve_f32_with_planner, correlate_f32_with_planner, convolve_f32_device_batch, correlate_f32_device_batch, f32,
+           PlannerConv32, phastft_conv_f32_host, phastft_conv_f32_dev);
+
+// ------------------------------------------------------------------------------------------------
 // r2c / c2r  (algorithms/r2c.rs:521-895)
 // ------------------------------------------------------------------------------------------------
 
@@ -516,6 +581,26 @@ mod interleaved {
                                r2c_fft_f32_interleaved_any_device_batch, c2r_fft_f32_interleaved_any_device_batch, f32, PlannerR2cAny32,
                                phastft_r2c_interleaved_any_f32_host, phastft_c2r_interleaved_any_f32_host,
                                phastft_r2c_interleaved_any_f32_dev, phastft_c2r_interleaved_any_f32_dev);
+
+    macro_rules! impl_conv_complex {
+        ($conv:ident, $corr:ident, $t:ty, $planner:ident, $ffi_host:ident) => {
+            /// Complex operands of a complex planner: `y` gets the window of `mode` of x * h.  Panics on a length mismatch,
+            /// and when the planner was built for real operands.
+            pub fn $conv(x: &[Complex<$t>], h: &[Complex<$t>], y: &mut [Complex<$t>], mode: ConvMode, planner: &$planner) {
+                check_conv_domain(planner.is_complex(), true);
+                check(unsafe { ffi::$ffi_host(planner.raw, CONV_CONVOLVE, mode as i32, x.as_ptr() as *const $t, x.len(),
+                                              h.as_ptr() as *const $t, h.len(), y.as_mut_ptr() as *mut $t, y.len()) });
+            }
+            /// The cross-correlation of x with h (convolution with conj(h) reversed), as the convolution, with its panics.
+            pub fn $corr(x: &[Complex<$t>], h: &[Complex<$t>], y: &mut [Complex<$t>], mode: ConvMode, planner: &$planner) {
+                check_conv_domain(planner.is_complex(), true);
+                check(unsafe { ffi::$ffi_host(planner.raw, CONV_CORRELATE, mode as i32, x.as_ptr() as *const $t, x.len(),
+                                              h.as_ptr() as *const $t, h.len(), y.as_mut_ptr() as *mut $t, y.len()) });
+            }
+        };
+    }
+    impl_conv_complex!(convolve_complex_f64_with_planner, correlate_complex_f64_with_planner, f64, PlannerConv64, phastft_conv_f64_host);
+    impl_conv_complex!(convolve_complex_f32_with_planner, correlate_complex_f32_with_planner, f32, PlannerConv32, phastft_conv_f32_host);
 }
 #[cfg(feature = "complex-nums")]
 pub use interleaved::*;

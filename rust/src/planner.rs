@@ -246,3 +246,62 @@ impl_planner_dct!(PlannerDct64, ffi::phastft_plan_dct_f64, phastft_plan_dct_f64_
                   phastft_plan_dct_f64_size, phastft_plan_dct_f64_describe, phastft_plan_dct_f64_reserve);
 impl_planner_dct!(PlannerDct32, ffi::phastft_plan_dct_f32, phastft_plan_dct_f32_create_with, phastft_plan_dct_f32_destroy,
                   phastft_plan_dct_f32_size, phastft_plan_dct_f32_describe, phastft_plan_dct_f32_reserve);
+
+macro_rules! impl_planner_conv {
+    ($name:ident, $raw:ty, $create:ident, $destroy:ident, $fft_len:ident, $describe:ident, $reserve:ident) => {
+        /// Additive: linear convolution and cross-correlation (scipy.signal.fftconvolve / correlate) of `n_x` values with
+        /// `n_h` values, real or complex, over an L-point transform, L = 2^ceil(log2(n_x + n_h - 1)) but at least 4.
+        pub struct $name {
+            pub(crate) raw: *mut $raw,
+            n_x: usize,
+            n_h: usize,
+            complex: bool,
+        }
+        unsafe impl Send for $name {}
+        unsafe impl Sync for $name {}
+        impl $name {
+            /// `complex`: the operands are interleaved complex values.  Panics for `n_x == 0`, `n_h == 0`, or L above 2^31
+            /// (real) / 2^30 (complex).
+            pub fn new(n_x: usize, n_h: usize, complex: bool) -> Self {
+                let mut raw = std::ptr::null_mut();
+                check(unsafe { ffi::$create(n_x, n_h, complex as std::os::raw::c_int, device(), &mut raw) });
+                Self { raw, n_x, n_h, complex }
+            }
+            pub fn n_x(&self) -> usize {
+                self.n_x
+            }
+            pub fn n_h(&self) -> usize {
+                self.n_h
+            }
+            pub fn is_complex(&self) -> bool {
+                self.complex
+            }
+            /// L, the length of the transforms the planner runs.
+            pub fn fft_len(&self) -> usize {
+                unsafe { ffi::$fft_len(self.raw) }
+            }
+            /// The output length of `mode`: n_x + n_h - 1, n_x or |n_x - n_h| + 1.
+            pub fn out_len(&self, mode: crate::ConvMode) -> usize {
+                unsafe { ffi::phastft_conv_out_len(self.n_x, self.n_h, mode as std::os::raw::c_int) }
+            }
+            /// `"n_x=<n_x> n_h=<n_h> f64 conv real L=2^<k> | "` followed by the inner plan's describe().
+            pub fn describe(&self) -> String {
+                unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
+            }
+            /// Makes every allocation a call of `batch` pairwise members would make, so such calls can be captured in a CUDA
+            /// graph.
+            pub fn reserve(&self, batch: usize) {
+                check(unsafe { ffi::$reserve(self.raw, batch) });
+            }
+        }
+        impl Drop for $name {
+            fn drop(&mut self) {
+                unsafe { ffi::$destroy(self.raw) }
+            }
+        }
+    };
+}
+impl_planner_conv!(PlannerConv64, ffi::phastft_plan_conv_f64, phastft_plan_conv_f64_create, phastft_plan_conv_f64_destroy,
+                   phastft_plan_conv_f64_fft_len, phastft_plan_conv_f64_describe, phastft_plan_conv_f64_reserve);
+impl_planner_conv!(PlannerConv32, ffi::phastft_plan_conv_f32, phastft_plan_conv_f32_create, phastft_plan_conv_f32_destroy,
+                   phastft_plan_conv_f32_fft_len, phastft_plan_conv_f32_describe, phastft_plan_conv_f32_reserve);
