@@ -110,6 +110,17 @@ template <> struct Api<double> {
     static int32_t conv_reserve(const Conv* p, std::size_t b) { return phastft_plan_conv_f64_reserve(p, b); }
     static int32_t conv_dev(const Conv* p, int op, int m, const double* x, std::size_t xs, const double* h, std::size_t hs, double* y, std::size_t ys, std::size_t b, void* s) { return phastft_conv_f64_dev(p, op, m, x, xs, h, hs, y, ys, b, s); }
     static int32_t conv_host(const Conv* p, int op, int m, const double* x, std::size_t lx, const double* h, std::size_t lh, double* y, std::size_t ly) { return phastft_conv_f64_host(p, op, m, x, lx, h, lh, y, ly); }
+    using Stft = phastft_plan_stft_f64;
+    static int32_t stft_create(std::size_t n, std::size_t nf, std::size_t hop, const double* w, std::size_t wl, int c, int pm, int dom, int dev, Stft** o) { return phastft_plan_stft_f64_create(n, nf, hop, w, wl, c, pm, dom, dev, o); }
+    static void stft_destroy(Stft* p) { phastft_plan_stft_f64_destroy(p); }
+    static std::size_t stft_frames(const Stft* p) { return phastft_plan_stft_f64_frames(p); }
+    static std::size_t stft_bins(const Stft* p) { return phastft_plan_stft_f64_bins(p); }
+    static const char* stft_describe(const Stft* p) { return phastft_plan_stft_f64_describe(p); }
+    static int32_t stft_reserve(const Stft* p, std::size_t b) { return phastft_plan_stft_f64_reserve(p, b); }
+    static int32_t stft_dev(const Stft* p, int nz, const double* x, std::size_t xs, double* s, std::size_t fs, std::size_t b, void* st) { return phastft_stft_f64_dev(p, nz, x, xs, s, fs, b, st); }
+    static int32_t istft_dev(const Stft* p, int nz, const double* s, std::size_t fs, double* y, std::size_t ys, std::size_t b, void* st) { return phastft_istft_f64_dev(p, nz, s, fs, y, ys, b, st); }
+    static int32_t stft_host(const Stft* p, int nz, const double* x, std::size_t lx, double* s, std::size_t ls) { return phastft_stft_f64_host(p, nz, x, lx, s, ls); }
+    static int32_t istft_host(const Stft* p, int nz, const double* s, std::size_t ls, double* y, std::size_t ly) { return phastft_istft_f64_host(p, nz, s, ls, y, ly); }
 };
 template <> struct Api<float> {
     using Dit = phastft_plan_dit_f32; using R2c = phastft_plan_r2c_f32;
@@ -171,6 +182,17 @@ template <> struct Api<float> {
     static int32_t conv_reserve(const Conv* p, std::size_t b) { return phastft_plan_conv_f32_reserve(p, b); }
     static int32_t conv_dev(const Conv* p, int op, int m, const float* x, std::size_t xs, const float* h, std::size_t hs, float* y, std::size_t ys, std::size_t b, void* s) { return phastft_conv_f32_dev(p, op, m, x, xs, h, hs, y, ys, b, s); }
     static int32_t conv_host(const Conv* p, int op, int m, const float* x, std::size_t lx, const float* h, std::size_t lh, float* y, std::size_t ly) { return phastft_conv_f32_host(p, op, m, x, lx, h, lh, y, ly); }
+    using Stft = phastft_plan_stft_f32;
+    static int32_t stft_create(std::size_t n, std::size_t nf, std::size_t hop, const float* w, std::size_t wl, int c, int pm, int dom, int dev, Stft** o) { return phastft_plan_stft_f32_create(n, nf, hop, w, wl, c, pm, dom, dev, o); }
+    static void stft_destroy(Stft* p) { phastft_plan_stft_f32_destroy(p); }
+    static std::size_t stft_frames(const Stft* p) { return phastft_plan_stft_f32_frames(p); }
+    static std::size_t stft_bins(const Stft* p) { return phastft_plan_stft_f32_bins(p); }
+    static const char* stft_describe(const Stft* p) { return phastft_plan_stft_f32_describe(p); }
+    static int32_t stft_reserve(const Stft* p, std::size_t b) { return phastft_plan_stft_f32_reserve(p, b); }
+    static int32_t stft_dev(const Stft* p, int nz, const float* x, std::size_t xs, float* s, std::size_t fs, std::size_t b, void* st) { return phastft_stft_f32_dev(p, nz, x, xs, s, fs, b, st); }
+    static int32_t istft_dev(const Stft* p, int nz, const float* s, std::size_t fs, float* y, std::size_t ys, std::size_t b, void* st) { return phastft_istft_f32_dev(p, nz, s, fs, y, ys, b, st); }
+    static int32_t stft_host(const Stft* p, int nz, const float* x, std::size_t lx, float* s, std::size_t ls) { return phastft_stft_f32_host(p, nz, x, lx, s, ls); }
+    static int32_t istft_host(const Stft* p, int nz, const float* s, std::size_t ls, float* y, std::size_t ly) { return phastft_istft_f32_host(p, nz, s, ls, y, ly); }
 };
 
 /// planner.rs:34-114
@@ -425,6 +447,78 @@ class PlannerConv {
     std::size_t n_x_ = 0, n_h_ = 0;
     bool cplx_ = false;
 };
+
+/// additive: the short-time Fourier transform and its inverse (torch.stft(..., return_complex=True) / torch.istft(..., length=n))
+/// of signals of n values, real or complex, over the n_fft-point plan: frames hop apart, the window's win_length values (empty:
+/// ones) centred in n_fft, and with `center` n_fft / 2 values of reflect or zero padding on each side
+enum class StftPad : int { Reflect = PHASTFT_STFT_PAD_REFLECT, Constant = PHASTFT_STFT_PAD_CONSTANT };
+template <typename T>
+class PlannerStft {
+  public:
+    /// `window` of win_length values, or empty for ones of win_length (0: n_fft); `complex_domain`: the signals are
+    /// std::complex<T> and the frames two-sided
+    PlannerStft(std::size_t n, std::size_t n_fft, std::size_t hop, const std::vector<T>& window = {}, std::size_t win_length = 0,
+                bool center = true, StftPad pad = StftPad::Reflect, int device = 0, bool complex_domain = false)
+        : n_(n), cplx_(complex_domain) {
+        const std::size_t wl = window.empty() ? (win_length ? win_length : n_fft) : window.size();
+        check(Api<T>::stft_create(n, n_fft, hop, window.empty() ? nullptr : window.data(), wl, center ? 1 : 0, static_cast<int>(pad),
+                                  complex_domain ? PHASTFT_STFT_COMPLEX : PHASTFT_STFT_REAL, device, &raw_));
+    }
+    ~PlannerStft() { if (raw_) Api<T>::stft_destroy(raw_); }
+    PlannerStft(PlannerStft&& o) noexcept : raw_(o.raw_), n_(o.n_), cplx_(o.cplx_) { o.raw_ = nullptr; }
+    PlannerStft(const PlannerStft&) = delete;
+    PlannerStft& operator=(const PlannerStft&) = delete;
+    std::size_t n() const { return n_; }
+    bool complex_domain() const { return cplx_; }
+    std::size_t frames() const { return Api<T>::stft_frames(raw_); }
+    std::size_t bins() const { return Api<T>::stft_bins(raw_); }
+    /// "n=<n> n_fft=<n_fft> hop=<hop> <prec> stft <real|complex> F=<F> | " followed by the inner plan's description
+    std::string describe() const { return Api<T>::stft_describe(raw_); }
+    /// make every allocation a call of `batch` signals would make now
+    void reserve(std::size_t batch) const { check(Api<T>::stft_reserve(raw_, batch)); }
+    /// real signal on host vectors: spec gets frames() x bins() values, frame-major (spec.size() == frames() * bins()).
+    /// Throws Panic on a length mismatch, and when the planner was built for complex signals.
+    void stft(const std::vector<T>& x, std::vector<std::complex<T>>& spec, bool normalized = false) const {
+        check_domain(false);
+        check(Api<T>::stft_host(raw_, normalized, x.data(), x.size(), reinterpret_cast<T*>(spec.data()), spec.size()));
+    }
+    void stft(const std::vector<std::complex<T>>& x, std::vector<std::complex<T>>& spec, bool normalized = false) const {
+        check_domain(true);
+        check(Api<T>::stft_host(raw_, normalized, reinterpret_cast<const T*>(x.data()), x.size(), reinterpret_cast<T*>(spec.data()),
+                                spec.size()));
+    }
+    /// the inverse of frame-major frames() x bins() values into n() values
+    void istft(const std::vector<std::complex<T>>& spec, std::vector<T>& y, bool normalized = false) const {
+        check_domain(false);
+        check(Api<T>::istft_host(raw_, normalized, reinterpret_cast<const T*>(spec.data()), spec.size(), y.data(), y.size()));
+    }
+    void istft(const std::vector<std::complex<T>>& spec, std::vector<std::complex<T>>& y, bool normalized = false) const {
+        check_domain(true);
+        check(Api<T>::istft_host(raw_, normalized, reinterpret_cast<const T*>(spec.data()), spec.size(), reinterpret_cast<T*>(y.data()),
+                                 y.size()));
+    }
+    /// `batch` signals on device pointers: member b at d_x + b * x_stride values (complex ones, as T pairs aligned to
+    /// 2 * sizeof(T), for a complex planner), frame f of member b at d_spec + (b * frames() + f) * frame_stride complex values
+    void stft_device(const T* d_x, std::size_t x_stride, T* d_spec, std::size_t frame_stride, std::size_t batch, bool normalized = false,
+                     void* stream = nullptr) const {
+        check(Api<T>::stft_dev(raw_, normalized, d_x, x_stride, d_spec, frame_stride, batch, stream));
+    }
+    void istft_device(const T* d_spec, std::size_t frame_stride, T* d_y, std::size_t y_stride, std::size_t batch, bool normalized = false,
+                      void* stream = nullptr) const {
+        check(Api<T>::istft_dev(raw_, normalized, d_spec, frame_stride, d_y, y_stride, batch, stream));
+    }
+  private:
+    // the host entry counts signal lengths in values of the planner's domain, so vectors of the other domain must not reach it
+    void check_domain(bool complex_signal) const {
+        if (complex_signal != cplx_)
+            throw Panic(PHASTFT_ERR_INVALID_ARG, std::string("PlannerStft domain mismatch: the planner was built for ") +
+                                                     (cplx_ ? "complex" : "real") + " signals, the vector is " +
+                                                     (complex_signal ? "complex" : "real"));
+    }
+    typename Api<T>::Stft* raw_ = nullptr;
+    std::size_t n_ = 0;
+    bool cplx_ = false;
+};
 }  // namespace detail
 
 using PlannerDit64 = detail::PlannerDit<double>;
@@ -444,6 +538,9 @@ using ConvMode = detail::ConvMode;
 using PlannerConv64 = detail::PlannerConv<double>;
 using PlannerConv32 = detail::PlannerConv<float>;
 using detail::conv_out_len;
+using StftPad = detail::StftPad;
+using PlannerStft64 = detail::PlannerStft<double>;
+using PlannerStft32 = detail::PlannerStft<float>;
 
 // ---- c2c (lib.rs:143-226, algorithms/dit.rs:263,338): in place on planar vectors -----------------------
 inline void fft_64_dit_with_planner_and_opts(std::vector<double>& reals, std::vector<double>& imags, Direction d, const PlannerDit64& p, const Options&) {

@@ -20,6 +20,8 @@ int main() {
     fails += !panics_with([] { PlannerR2c64 p(6); }, "n must be a power of 2 >= 4");
     fails += !panics_with([] { PlannerDct64 p(0); }, "n must be >= 1");
     fails += !panics_with([] { PlannerConv64 p(0, 5); }, "n_x and n_h must be >= 1");
+    fails += !panics_with([] { PlannerStft64 p(32, 64, 16); }, "reflect padding");
+    fails += !panics_with([] { PlannerStft32 p(100, 64, 0); }, "hop must be >= 1");
     fails += !panics_with([] { PlannerConv32 p(std::size_t(1) << 30, 2, 0, true); }, "above 2^30");
     fails += conv_out_len(10, 4, ConvMode::Full) != 13 || conv_out_len(10, 4, ConvMode::Same) != 10 || conv_out_len(4, 10, ConvMode::Valid) != 7;
     fails += !panics_with([] { std::vector<float> x(2), a(2), b(2); r2c_fft_f32(x, a, b); }, "n must be a power of 2 >= 4");
@@ -86,6 +88,27 @@ int main() {
             for (std::size_t k = 0; k < nh; ++k) s += std::complex<double>(cx[j + k]) * std::conj(std::complex<double>(ch[k]));
             fails += std::abs(std::complex<double>(cy[j]) - s) > 1e-4;
         }
+    }
+    {   // additive surface: a round trip through the STFT, real and complex
+        const std::size_t n = 4000, nf = 400, hop = 100;
+        std::vector<double> w(nf);
+        for (std::size_t i = 0; i < nf; ++i) w[i] = 0.5 - 0.5 * std::cos(2 * 3.14159265358979323846 * i / nf);
+        PlannerStft64 p(n, nf, hop, w);
+        fails += p.frames() != 41 || p.bins() != 201 || p.describe().find("n=4000 n_fft=400 hop=100 f64 stft real F=41 | ") != 0;
+        std::vector<double> x(n), y(n);
+        for (std::size_t i = 0; i < n; ++i) x[i] = std::sin(0.37 * i);
+        std::vector<std::complex<double>> spec(p.frames() * p.bins());
+        p.stft(x, spec);
+        p.istft(spec, y);
+        for (std::size_t i = 0; i < n; ++i) fails += std::fabs(y[i] - x[i]) > 1e-12;
+        fails += !panics_with([&] { std::vector<std::complex<double>> c(n); p.stft(c, spec); }, "domain mismatch");
+        PlannerStft32 q(n, 512, 128, {}, 0, false, StftPad::Constant, 0, true);
+        std::vector<std::complex<float>> cx(n), cy(n), cs(q.frames() * q.bins());
+        for (std::size_t i = 0; i < n; ++i) cx[i] = {std::sin(0.37f * i), std::cos(0.5f * i)};
+        q.stft(cx, cs);
+        q.istft(cs, cy);
+        const std::size_t covered = 512 + 128 * (q.frames() - 1);
+        for (std::size_t i = 0; i < covered; ++i) fails += std::abs(cy[i] - cx[i]) > 1e-5f;
     }
     std::printf("gpu checks: %d failures\n", fails);
     return fails;

@@ -56,7 +56,7 @@ PHASTFT_API uint64_t phastft_launch_count(void);
  * CHIRP-POST-R2C-IL / CHIRP-PRE-C2R-IL / SMOOTH-PRE-C2R-IL / ODD-R2C-IL / SMOOTH-POST-R2C-IL (the spectrum's end of
  * phastft_{r2c,c2r}_interleaved_any_*, whose halved mixed r2c's last pass is ODD-IL), DCT-PRE-<kind> / DCT-POST-<kind> (the ends of
  * phastft_dct_*, kind DCT2, DCT3, DST2 or DST3: R=<N>, C=<members>), CONV-PRE / CONV-MUL / CONV-POST (phastft_conv_*: R=<L>,
- * C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
+ * C=<members>), STFT-FRAME (phastft_stft_*: R=<n_fft>, C=<frames>) / ISTFT-OLA (phastft_istft_*: R=<n_fft>, C=<members>); mode plain, tma (tile input by TMA), bulk (tile input by bulk copies), row-bulk (one-CTA tile in and out by bulk
  * copies), c2r-in (c2r pre-processing on load), c2r-in-il (the same from interleaved bins), cluster, pipe or pipe-tma; " pdl" marks
  * programmatic dependent launch.
  * Reset at the start of every execution call; valid until the thread's next call. */
@@ -552,6 +552,67 @@ PHASTFT_API int32_t phastft_conv_f64_host(const phastft_plan_conv_f64* plan, int
                                           const double* h, size_t len_h, double* y, size_t len_y);
 PHASTFT_API int32_t phastft_conv_f32_host(const phastft_plan_conv_f32* plan, int op, int mode, const float* x, size_t len_x,
                                           const float* h, size_t len_h, float* y, size_t len_y);
+
+/* ---- short-time Fourier transform and its inverse of real or complex signals (torch.stft / torch.istft) -------------------
+ * The semantics of torch.stft(x, n_fft, hop, win_length, window, center, pad_mode, normalized, return_complex=True) and
+ * torch.istft(spec, n_fft, hop, win_length, window, center, normalized, length=n) for signals of n values.
+ * _create: `window` is win_length host values (NULL: ones), zero-padded to n_fft from (n_fft - win_length) / 2 and kept on the
+ * device in the plan's precision.  center pads n_fft / 2 values on each side, by reflection (PHASTFT_STFT_PAD_REFLECT) or
+ * zeros (PHASTFT_STFT_PAD_CONSTANT).  F = 1 + (n + 2 pad - n_fft) / hop frames (_frames) of n_fft / 2 + 1 bins (domain
+ * PHASTFT_STFT_REAL) or n_fft bins (PHASTFT_STFT_COMPLEX) (_bins), on the n_fft-point real or complex any-length plan
+ * (PHASTFT_ANY_AUTO).  n or n_fft of 0, hop == 0, win_length of 0 or above n_fft, reflect padding with n_fft / 2 >= n, n <
+ * n_fft without center, a bad pad mode or domain, and anything the inner plan refuses return PHASTFT_ERR_INVALID_ARG before the
+ * device is touched.  _create also runs torch's NOLA check in long double (the window-squared overlap-add envelope >= 1e-11
+ * over every retained sample some frame covers) and records the result: the STFT always runs; the istft of a failing plan
+ * returns PHASTFT_ERR_INVALID_ARG naming the first failing sample.
+ * describe() is "n=<n> n_fft=<n_fft> hop=<hop> <prec> stft <real|complex> F=<F> | " followed by the inner plan's describe().
+ * _dev: member b's n values at d_x (d_y) + b * x_stride (y_stride); frame f of member b at d_spec + (b * F + f) * frame_stride
+ * complex values (torch's layout; frame_stride >= the bin count).  Real signals: any element offsets; complex ones: interleaved
+ * pairs, strides in complex values.  d_spec (and complex signals) aligned to 2 * sizeof(T).  normalized other than 0 / 1, NULL
+ * or misaligned pointers, a short frame_stride, x_stride / y_stride < n with batch > 1, or d_spec's frames overlapping the
+ * signals return PHASTFT_ERR_INVALID_ARG before any launch; batch == 0 does nothing.  The stft writes no value between frames;
+ * the istft never writes d_spec and writes zero where no frame covers a sample (torch's tail).  Launches: STFT-FRAME, then the
+ * inner forward launches over batch x F frames; the inner inverse launches, then ISTFT-OLA (complex: a strided device copy of
+ * the frames into the workspace comes first).  The workspace follows the any-length plans' protocol (_reserve(batch) grows it
+ * and the inner plan's for batch x F frames; capturing without it fails naming phastft_plan_stft_*_reserve).
+ * _host: synchronous through a plan-owned staging buffer; dense frames (F x bins complex values); len_x / len_spec (stft) or
+ * len_spec (istft) wrong is PHASTFT_ERR_INPUT_LEN, the output length wrong PHASTFT_ERR_OUTPUT_LEN. */
+#define PHASTFT_STFT_REAL 0
+#define PHASTFT_STFT_COMPLEX 1
+#define PHASTFT_STFT_PAD_REFLECT 0
+#define PHASTFT_STFT_PAD_CONSTANT 1
+typedef struct phastft_plan_stft_f64 phastft_plan_stft_f64;
+typedef struct phastft_plan_stft_f32 phastft_plan_stft_f32;
+PHASTFT_API int32_t phastft_plan_stft_f64_create(size_t n, size_t n_fft, size_t hop, const double* window, size_t win_length, int center,
+                                                 int pad_mode, int domain, int device, phastft_plan_stft_f64** out);
+PHASTFT_API int32_t phastft_plan_stft_f32_create(size_t n, size_t n_fft, size_t hop, const float* window, size_t win_length, int center,
+                                                 int pad_mode, int domain, int device, phastft_plan_stft_f32** out);
+PHASTFT_API void phastft_plan_stft_f64_destroy(phastft_plan_stft_f64* plan);
+PHASTFT_API void phastft_plan_stft_f32_destroy(phastft_plan_stft_f32* plan);
+PHASTFT_API size_t phastft_plan_stft_f64_frames(const phastft_plan_stft_f64* plan);
+PHASTFT_API size_t phastft_plan_stft_f32_frames(const phastft_plan_stft_f32* plan);
+PHASTFT_API size_t phastft_plan_stft_f64_bins(const phastft_plan_stft_f64* plan);
+PHASTFT_API size_t phastft_plan_stft_f32_bins(const phastft_plan_stft_f32* plan);
+PHASTFT_API const char* phastft_plan_stft_f64_describe(const phastft_plan_stft_f64* plan);
+PHASTFT_API const char* phastft_plan_stft_f32_describe(const phastft_plan_stft_f32* plan);
+PHASTFT_API int32_t phastft_plan_stft_f64_reserve(const phastft_plan_stft_f64* plan, size_t batch);
+PHASTFT_API int32_t phastft_plan_stft_f32_reserve(const phastft_plan_stft_f32* plan, size_t batch);
+PHASTFT_API int32_t phastft_stft_f64_dev(const phastft_plan_stft_f64* plan, int normalized, const double* d_x, size_t x_stride, double* d_spec,
+                                         size_t frame_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_stft_f32_dev(const phastft_plan_stft_f32* plan, int normalized, const float* d_x, size_t x_stride, float* d_spec,
+                                         size_t frame_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_istft_f64_dev(const phastft_plan_stft_f64* plan, int normalized, const double* d_spec, size_t frame_stride,
+                                          double* d_y, size_t y_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_istft_f32_dev(const phastft_plan_stft_f32* plan, int normalized, const float* d_spec, size_t frame_stride,
+                                          float* d_y, size_t y_stride, size_t batch, void* stream);
+PHASTFT_API int32_t phastft_stft_f64_host(const phastft_plan_stft_f64* plan, int normalized, const double* x, size_t len_x, double* spec,
+                                          size_t len_spec);
+PHASTFT_API int32_t phastft_stft_f32_host(const phastft_plan_stft_f32* plan, int normalized, const float* x, size_t len_x, float* spec,
+                                          size_t len_spec);
+PHASTFT_API int32_t phastft_istft_f64_host(const phastft_plan_stft_f64* plan, int normalized, const double* spec, size_t len_spec,
+                                           double* y, size_t len_y);
+PHASTFT_API int32_t phastft_istft_f32_host(const phastft_plan_stft_f32* plan, int normalized, const float* spec, size_t len_spec,
+                                           float* y, size_t len_y);
 
 /* ---- lib.rs:41-140 (feature complex-nums): fft_{64,32}_interleaved* --------------------------
  * signal = N interleaved (re, im) pairs (num_complex::Complex<T> layout), in place.  The

@@ -145,6 +145,16 @@ SIGNATURES = {
     "phastft_plan_conv_{s}_reserve": ([_vp, _sz], _i32),
     "phastft_conv_{s}_dev": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
     "phastft_conv_{s}_host": ([_vp, _ci, _ci, _vp, _sz, _vp, _sz, _vp, _sz], _i32),
+    "phastft_plan_stft_{s}_create": ([_sz, _sz, _sz, _vp, _sz, _ci, _ci, _ci, _ci, C.POINTER(_vp)], _i32),
+    "phastft_plan_stft_{s}_destroy": ([_vp], None),
+    "phastft_plan_stft_{s}_frames": ([_vp], _sz),
+    "phastft_plan_stft_{s}_bins": ([_vp], _sz),
+    "phastft_plan_stft_{s}_describe": ([_vp], C.c_char_p),
+    "phastft_plan_stft_{s}_reserve": ([_vp, _sz], _i32),
+    "phastft_stft_{s}_dev": ([_vp, _ci, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_istft_{s}_dev": ([_vp, _ci, _vp, _sz, _vp, _sz, _sz, _vp], _i32),
+    "phastft_stft_{s}_host": ([_vp, _ci, _vp, _sz, _vp, _sz], _i32),
+    "phastft_istft_{s}_host": ([_vp, _ci, _vp, _sz, _vp, _sz], _i32),
 }
 def check(code: int):
     if code != OK:

@@ -49,6 +49,7 @@ __all__ = [
     "PlannerDct64", "PlannerDct32", "dct_f64_with_planner", "dct_f32_with_planner", "dst_f64_with_planner", "dst_f32_with_planner",
     "dct_batch", "dst_batch",
     "PlannerConv64", "PlannerConv32", "convolve_with_planner", "correlate_with_planner", "convolve_batch", "correlate_batch",
+    "PlannerStft64", "PlannerStft32", "stft_with_planner", "istft_with_planner", "stft_batch", "istft_batch",
 ]
 
 
@@ -1340,3 +1341,243 @@ def correlate_batch(x, h, out, planner, batch: int, mode: str = "full", x_stride
                     out_stride: int | None = None) -> None:
     """convolve_batch for scipy.signal.correlate."""
     _conv_batch(1, x, h, out, planner, batch, mode, x_stride, h_stride, out_stride)
+
+
+# ----------------------------------------------------------------------------------------------
+# short-time Fourier transform and its inverse (torch.stft(..., return_complex=True) / torch.istft(..., length=n))
+# ----------------------------------------------------------------------------------------------
+_STFT_PAD = {"reflect": 0, "constant": 1}
+
+
+class _PlannerStft:
+    _sfx = ""
+    _dtype = None
+
+    def __init__(self, n: int, n_fft: int, hop_length: int | None = None, win_length: int | None = None, window=None,
+                 center: bool = True, pad_mode: str = "reflect", device: int = 0, complex: bool = False):
+        """torch.stft / torch.istft of signals of n values (real, or interleaved complex128 / complex64 with complex=True):
+        frames of n_fft values hop_length apart (default n_fft // 4), the window's win_length values (default n_fft; window
+        None: ones) centred in n_fft, and with center the signal padded by n_fft // 2 values on each side (pad_mode "reflect"
+        or "constant").  n_frames frames of n_bins bins (n_fft // 2 + 1 real, n_fft complex).  A bad pad_mode or a window of
+        another length raises ValueError; what the library refuses (hop 0, win_length above n_fft, reflect padding of n_fft // 2
+        >= n, n < n_fft without center, ...) raises PhastFTPanic(13) before the device is touched."""
+        self._h = C.c_void_p()
+        n_fft = int(n_fft)
+        hop_length = n_fft // 4 if hop_length is None else int(hop_length)
+        win_length = n_fft if win_length is None else int(win_length)
+        if not isinstance(pad_mode, str) or pad_mode not in _STFT_PAD:
+            raise ValueError(f"pad_mode must be 'reflect' or 'constant', got {pad_mode!r}")
+        w = None
+        if window is not None:
+            if _is_torch(window):
+                window = window.detach().cpu().numpy()
+            w = np.ascontiguousarray(np.asarray(window, dtype=self._dtype))
+            if w.ndim != 1 or w.size != win_length:
+                raise ValueError(f"window must be 1-D with win_length = {win_length} values, got shape {w.shape}")
+        self.device = int(device)
+        self.complex = bool(complex)
+        check(fn("phastft_plan_stft_{s}_create", self._sfx)(int(n), n_fft, hop_length,
+                                                           None if w is None else w.ctypes.data_as(C.c_void_p), win_length,
+                                                           int(bool(center)), _STFT_PAD[pad_mode], int(self.complex), self.device,
+                                                           C.byref(self._h)))
+        self.n, self.n_fft, self.hop_length, self.win_length = int(n), n_fft, hop_length, win_length
+        self.center, self.pad_mode = bool(center), pad_mode
+
+    @property
+    def n_frames(self) -> int:
+        """F = 1 + (n + 2 pad - n_fft) // hop_length, pad = n_fft // 2 with center, else 0."""
+        return int(fn("phastft_plan_stft_{s}_frames", self._sfx)(self._h))
+
+    @property
+    def n_bins(self) -> int:
+        """n_fft // 2 + 1 (real signals) or n_fft (complex)."""
+        return int(fn("phastft_plan_stft_{s}_bins", self._sfx)(self._h))
+
+    def describe(self) -> str:
+        """"n=<n> n_fft=<n_fft> hop=<hop> <prec> stft <real|complex> F=<F> | " followed by the inner plan's describe()."""
+        return fn("phastft_plan_stft_{s}_describe", self._sfx)(self._h).decode()
+
+    def reserve(self, batch: int) -> None:
+        """Make every allocation a call of `batch` signals would make now (otherwise the first larger call makes them,
+        synchronising the device -- an error inside a CUDA-graph capture)."""
+        check(fn("phastft_plan_stft_{s}_reserve", self._sfx)(self._h, int(batch)))
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        if h:
+            self._h = None
+            try:
+                fn("phastft_plan_stft_{s}_destroy", self._sfx)(h)
+            except (AttributeError, TypeError):      # interpreter shutdown: the module globals are already gone
+                pass
+
+
+class PlannerStft64(_PlannerStft):
+    _sfx, _dtype = "f64", np.float64
+
+
+class PlannerStft32(_PlannerStft):
+    _sfx, _dtype = "f32", np.float32
+
+
+def _stft_dtypes(planner):
+    """(signal dtype, spectrum dtype) as numpy dtypes"""
+    cdt = np.complex128 if planner._sfx == "f64" else np.complex64
+    return np.dtype(cdt if planner.complex else planner._dtype), np.dtype(cdt)
+
+
+def _torch_dtype(dt):
+    import torch
+    return {np.dtype(np.float64): torch.float64, np.dtype(np.float32): torch.float32,
+            np.dtype(np.complex128): torch.complex128, np.dtype(np.complex64): torch.complex64}[np.dtype(dt)]
+
+
+def _normalized(normalized) -> int:
+    if isinstance(normalized, (bool, np.bool_)) or normalized in (0, 1):
+        return int(bool(normalized))
+    raise ValueError(f"normalized must be a bool, got {normalized!r}")
+
+
+def _sig_stride(t, n: int):
+    """member stride of a (..., n) tensor whose last dimension is unit-stride and whose leading dimensions flatten to one
+    stride >= n, else None"""
+    if n > 1 and t.stride(-1) != 1:
+        return None
+    cands, inner = [], 1
+    for size, st in reversed(list(zip(t.shape[:-1], t.stride()[:-1]))):
+        if size > 1:
+            if st % inner:
+                return None
+            cands.append(st // inner)
+        inner *= size
+    s = cands[0] if cands else n
+    return s if s >= n and all(c == s for c in cands) else None
+
+
+def _frame_stride(t, bins: int, frames: int):
+    """frame stride fs of a (..., bins, F) spectrum whose element (b, k, f) lies at (b F + f) fs + k (torch.stft's layout, b
+    the flattened leading index, fs >= bins), else None"""
+    if bins > 1 and t.stride(-2) != 1:
+        return None
+    cands, inner = [], frames
+    if frames > 1:
+        cands.append(t.stride(-1))
+    for size, st in reversed(list(zip(t.shape[:-2], t.stride()[:-2]))):
+        if size > 1:
+            if st % inner:
+                return None
+            cands.append(st // inner)
+        inner *= size
+    fs = cands[0] if cands else bins
+    return fs if fs >= bins and all(c == fs for c in cands) else None
+
+
+def _stft_torch(inverse: bool, sig, spec, planner, normalized: int):
+    """One device call on torch CUDA tensors sig (..., n) and spec (..., n_bins, F) with the same leading shape.  A tensor in
+    another layout, or a complex one that is not aligned to its element size, goes through a temporary."""
+    import torch
+    sdt, cdt = _stft_dtypes(planner)
+    n, bins, F = planner.n, planner.n_bins, planner.n_frames
+    for what, t, want in (("signal", sig, sdt), ("spectrum", spec, cdt)):
+        if not _is_torch(t) or not t.is_cuda:
+            raise TypeError(f"{what}: pass both arrays as torch CUDA tensors, or both as numpy arrays")
+        if t.dtype != _torch_dtype(want):
+            raise ValueError(f"{what}: expected dtype {_torch_dtype(want)} for this planner, got {t.dtype}")
+    if sig.dim() < 1 or sig.shape[-1] != n:
+        raise ValueError(f"the signal has shape {tuple(sig.shape)}, the planner expects (..., {n})")
+    lead = tuple(sig.shape[:-1])
+    if tuple(spec.shape) != lead + (bins, F):
+        raise ValueError(f"the spectrum has shape {tuple(spec.shape)}, the planner expects {lead + (bins, F)}")
+    batch = int(np.prod(lead, dtype=np.int64)) if lead else 1
+
+    def aligned(t):
+        return not t.is_complex() or t.data_ptr() % t.element_size() == 0
+    ss = _sig_stride(sig, n) if aligned(sig) else None
+    fs = _frame_stride(spec, bins, F) if aligned(spec) else None
+    sig_w = sig if ss is not None else torch.empty((batch, n), dtype=sig.dtype, device=sig.device)
+    spec_w = spec if fs is not None else torch.empty((batch, F, bins), dtype=spec.dtype, device=spec.device).transpose(1, 2)
+    if inverse and fs is None:
+        spec_w.copy_(spec.reshape(batch, bins, F))
+    if not inverse and ss is None:
+        sig_w.copy_(sig.reshape(batch, n))
+    ss = n if ss is None else ss
+    fs = bins if fs is None else fs
+    name = "phastft_istft_{s}_dev" if inverse else "phastft_stft_{s}_dev"
+    a, b, sa, sb = (spec_w, sig_w, fs, ss) if inverse else (sig_w, spec_w, ss, fs)
+    check(fn(name, planner._sfx)(planner._h, normalized, C.c_void_p(a.data_ptr()), sa, C.c_void_p(b.data_ptr()), sb, batch,
+                                 _torch_stream(spec)))
+    if inverse and sig_w is not sig:
+        sig.copy_(sig_w.reshape(sig.shape))
+    if not inverse and spec_w is not spec:
+        spec.copy_(spec_w.reshape(spec.shape))
+
+
+def _stft_numpy(inverse: bool, sig, spec, planner, normalized: int):
+    """One synchronous host call on a 1-D numpy signal and an (n_bins, F) numpy spectrum."""
+    sdt, cdt = _stft_dtypes(planner)
+    n, bins, F = planner.n, planner.n_bins, planner.n_frames
+    for what, a, want in (("signal", sig, sdt), ("spectrum", spec, cdt)):
+        if not isinstance(a, np.ndarray):
+            raise TypeError(f"{what}: pass both arrays as torch CUDA tensors, or both as numpy arrays")
+        if a.dtype != want:
+            raise ValueError(f"{what}: expected dtype {want} for this planner, got {a.dtype}")
+    if sig.shape != (n,):
+        raise ValueError(f"the signal has shape {sig.shape}, the planner expects ({n},)")
+    if spec.shape != (bins, F):
+        raise ValueError(f"the spectrum has shape {spec.shape}, the planner expects ({bins}, {F})")
+    out = spec if not inverse else sig
+    if not out.flags.writeable:
+        raise ValueError("the output array is read-only")
+    direct = spec.T.flags.c_contiguous
+    frames = spec.T if direct else np.ascontiguousarray(spec.T)   # F x bins, dense
+    s = sig if sig.flags.c_contiguous else np.ascontiguousarray(sig)
+    if inverse:
+        check(fn("phastft_istft_{s}_host", planner._sfx)(planner._h, normalized, frames.ctypes.data_as(C.c_void_p), frames.size,
+                                                         s.ctypes.data_as(C.c_void_p), s.size))
+        if s is not sig:
+            sig[...] = s
+    else:
+        check(fn("phastft_stft_{s}_host", planner._sfx)(planner._h, normalized, s.ctypes.data_as(C.c_void_p), s.size,
+                                                        frames.ctypes.data_as(C.c_void_p), frames.size))
+        if not direct:
+            spec[...] = frames.T
+
+
+def _stft_call(inverse: bool, sig, spec, planner, normalized, batched: bool):
+    if not isinstance(planner, _PlannerStft):
+        raise TypeError("expected a PlannerStft64 or PlannerStft32")
+    nz = _normalized(normalized)
+    if _is_torch(sig) or _is_torch(spec):
+        if not batched and (getattr(sig, "dim", lambda: 0)() != 1):
+            raise ValueError("stft_with_planner / istft_with_planner take one signal: use stft_batch / istft_batch for more")
+        _stft_torch(inverse, sig, spec, planner, nz)
+    elif batched:
+        raise TypeError("stft_batch / istft_batch take torch CUDA tensors")
+    else:
+        _stft_numpy(inverse, sig, spec, planner, nz)
+
+
+def stft_with_planner(x, out, planner, normalized: bool = False) -> None:
+    """torch.stft(x, ..., return_complex=True) of one signal into out: x of n values (float64 / float32, or complex128 /
+    complex64 for a complex planner) and out of shape (n_bins, n_frames), complex.  numpy arrays (synchronous, through a
+    staging buffer) or torch CUDA tensors (torch's current stream); out in any other layout than torch.stft's (unit bin
+    stride) goes through a temporary."""
+    _stft_call(False, x, out, planner, normalized, False)
+
+
+def istft_with_planner(spec, out, planner, normalized: bool = False) -> None:
+    """torch.istft(spec, ..., length=n) of one spectrum of shape (n_bins, n_frames) into out of n values (real, or complex for
+    a complex planner); numpy arrays or torch CUDA tensors.  spec is not written.  A plan whose window fails the NOLA
+    condition raises PhastFTPanic(13) naming the first sample where the overlap-add envelope is below 1e-11."""
+    _stft_call(True, out, spec, planner, normalized, False)
+
+
+def stft_batch(x, out, planner, normalized: bool = False) -> None:
+    """stft_with_planner over torch CUDA tensors x (..., n) and out (..., n_bins, n_frames): one device call when out has
+    torch.stft's layout and the leading dimensions of each flatten to one stride."""
+    _stft_call(False, x, out, planner, normalized, True)
+
+
+def istft_batch(spec, out, planner, normalized: bool = False) -> None:
+    """istft_with_planner over torch CUDA tensors spec (..., n_bins, n_frames) and out (..., n)."""
+    _stft_call(True, out, spec, planner, normalized, True)

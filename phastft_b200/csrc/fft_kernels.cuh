@@ -1724,4 +1724,90 @@ __global__ void __launch_bounds__(256) conv_post_kernel(const __grid_constant__ 
     reinterpret_cast<E*>(p.y)[b * p.y_stride + j] = reinterpret_cast<const E*>(p.sig)[b * p.L + p.start + j];
 }
 
+// ---------------------------------------------------------------------------------------------
+// STFT-FRAME / ISTFT-OLA: the two elementwise kernels of the short-time Fourier transform (torch.stft / torch.istft) around
+// the n_fft-point real or complex plan.  Frame f of member b is global frame m = b * n_frames + f; it covers the samples
+// t = f * hop + j - pad (0 <= j < n_fft) of the member's signal, read with reflect or zero padding.  FRAME writes frame m at
+// frames + m * fstride (reals for real signals, (re, im) pairs for complex ones), each sample times win[j] (the window,
+// pre-scaled by n_fft^(-1/2) when normalized).  OLA writes output sample t of member b as
+//   sum_f win[j] v_f[j] / sum_f win[j]^2 * scale,   j = t + pad - f * hop,
+// over the frames that cover t + pad in ascending f (no atomics: bit-reproducible), zero where no frame does.  With EVEN_FIX
+// (real signals, even n_fft) it first removes from each frame sample what the c2r adds for the imaginary parts of bin 0 (a)
+// and bin n_fft / 2 (b), which numpy.fft.irfft and torch drop: -(a + b) / n_fft at even j, (a - b) / n_fft at odd j.  The
+// caller's arrays are accessed one element at a time.  A member-major grid of 256-thread blocks, member m0 + blockIdx.x /
+// blocks_per_member.
+template <typename T>
+struct StftParams {
+    const T* x;                    // FRAME: the caller's signals
+    T* frames;                     // FRAME: out, OLA: in; frame m at frames + m * fstride values (complex ones for CPLX)
+    const cx<T>* spec;             // OLA with EVEN_FIX: the caller's bins, frame m at spec + m * spec_stride
+    T* y;                          // OLA: the caller's output
+    const T* win;                  // n_fft window values
+    long long n, n_fft, hop, pad, n_frames;
+    long long x_stride, fstride, spec_stride, y_stride;   // in values (complex ones for complex signals)
+    long long m0;                  // the first member (FRAME: frame) of this launch
+    T scale;                       // OLA: sqrt(n_fft) when normalized, else 1
+    T inv_n;                       // OLA with EVEN_FIX: 1 / n_fft
+    int reflect;                   // FRAME: reflect padding, else zeros
+    unsigned blocks_per_member;
+};
+
+template <typename T, bool CPLX>
+__global__ void __launch_bounds__(256) stft_frame_kernel(const __grid_constant__ StftParams<T> p) {
+    using E = conv_value_t<T, CPLX>;
+    const long long m = p.m0 + blockIdx.x / p.blocks_per_member;
+    const long long j = (long long)(blockIdx.x % p.blocks_per_member) * 256 + threadIdx.x;
+    if (j >= p.n_fft) return;
+    const long long b = m / p.n_frames;
+    long long t = (m - b * p.n_frames) * p.hop + j - p.pad;
+    bool inside = true;
+    if (t < 0 || t >= p.n) {
+        if (p.reflect) t = t < 0 ? -t : 2 * (p.n - 1) - t;   // pad < n: one reflection lands inside
+        else inside = false;
+    }
+    const T w = p.win[j];
+    if constexpr (CPLX) {
+        cx<T> v = make_cx<T>(T(0), T(0));
+        if (inside) v = reinterpret_cast<const cx<T>*>(p.x)[b * p.x_stride + t];
+        reinterpret_cast<cx<T>*>(p.frames)[m * p.fstride + j] = make_cx<T>(v.x * w, v.y * w);
+    } else {
+        const T v = inside ? p.x[b * p.x_stride + t] : T(0);
+        p.frames[m * p.fstride + j] = v * w;
+    }
+}
+
+template <typename T, bool CPLX, bool EVEN_FIX>
+__global__ void __launch_bounds__(256) istft_ola_kernel(const __grid_constant__ StftParams<T> p) {
+    using E = conv_value_t<T, CPLX>;
+    const long long b = p.m0 + blockIdx.x / p.blocks_per_member;
+    const long long t = (long long)(blockIdx.x % p.blocks_per_member) * 256 + threadIdx.x;
+    if (t >= p.n) return;
+    const long long u = t + p.pad;
+    const long long f_hi = min(u / p.hop, p.n_frames - 1);
+    const long long f_lo = u >= p.n_fft ? (u - p.n_fft) / p.hop + 1 : 0;   // the first frame with u - f * hop < n_fft
+    T nre = T(0), nim = T(0), den = T(0);
+    for (long long f = f_lo; f <= f_hi; ++f) {
+        const long long j = u - f * p.hop, m = b * p.n_frames + f;
+        const T w = p.win[j];
+        if constexpr (CPLX) {
+            const cx<T> v = reinterpret_cast<const cx<T>*>(p.frames)[m * p.fstride + j];
+            nre += w * v.x;
+            nim += w * v.y;
+        } else {
+            T v = p.frames[m * p.fstride + j];
+            if constexpr (EVEN_FIX) {
+                const T* im = reinterpret_cast<const T*>(p.spec + m * p.spec_stride) + 1;   // Im X[0], Im X[n_fft / 2]
+                const T a = im[0], c = im[p.n_fft];
+                v -= ((j & 1) ? a - c : -(a + c)) * p.inv_n;
+            }
+            nre += w * v;
+        }
+        den += w * w;
+    }
+    E* y = reinterpret_cast<E*>(p.y) + b * p.y_stride + t;
+    const bool covered = f_lo <= f_hi;
+    if constexpr (CPLX) *y = covered ? make_cx<T>(nre / den * p.scale, nim / den * p.scale) : make_cx<T>(T(0), T(0));
+    else *y = covered ? nre / den * p.scale : T(0);
+}
+
 }  // namespace phast

@@ -3921,6 +3921,303 @@ int32_t conv_host(const PlanConv<T>* pl, int op, int mode, const T* x, size_t le
     return PHASTFT_OK;
 }
 
+// =================================================================================================
+// short-time Fourier transform and its inverse of real or complex signals (torch.stft(..., return_complex=True) /
+// torch.istft(..., length=n)): STFT-FRAME and the n_fft-point real plan's interleaved r2c (or the complex plan's forward
+// transform) over every frame of the batch; the c2r (or reverse transform) into workspace frames and ISTFT-OLA
+// (fft_kernels.cuh).  Frame f of member b is global frame b * F + f, frame_stride complex values apart in the caller's spectrum.
+// =================================================================================================
+template <typename T>
+struct PlanStft {
+    size_t n = 0, n_fft = 0, hop = 0, pad = 0, frames = 0, bins = 0;   // frames: F per member
+    int device = 0;
+    bool cplx = false, reflect = true;
+    PlanR2cAny<T>* real = nullptr;     // real signals: the n_fft-point real plan
+    PlanAny<T>* cinner = nullptr;      // complex signals: the n_fft-point complex plan
+    T* win = nullptr;                  // 2 x n_fft: the window zero-padded to n_fft, then the same times n_fft^(-1/2)
+    long long nola_fail = -1;          // the first retained sample whose overlap-add envelope is below 1e-11, or -1
+    long double nola_env = 0;          // its envelope
+    // per call of B members: B x F frames of fstride() reals (real) or n_fft complex values (complex; istft only).  The
+    // AnyWorkspace protocol.
+    mutable AnyWorkspace<T> w;
+    mutable std::mutex host_mu;        // held for a whole *_host call (lock order: host_mu, then w.mu, then the inner plan's)
+    mutable T* stage = nullptr;        // host-API staging: F x bins complex values, then n signal values; allocated by the first host call
+    std::string description;
+    size_t fstride() const { return cplx ? n_fft : n_fft + (n_fft & 1); }   // workspace frame stride in values: even for reals,
+    size_t member_elems() const { return cplx ? n_fft : fstride() / 2; }     // so the inner r2c / c2r may access them as pairs
+    size_t vals() const { return cplx ? 2 : 1; }                             // T per signal value
+    size_t stage_elems() const { return 2 * frames * bins + vals() * n; }    // T
+    cudaStream_t host_stream() const {
+        if (cplx) return cinner->pow2 ? cinner->pow2->stream : cinner->host_stream();
+        return real->pow2 ? real->pow2->inner->stream : real->host_stream();
+    }
+    ~PlanStft() {
+        DeviceGuard g(device);
+        w.destroy();
+        for (void* p : {(void*)win, (void*)stage})
+            if (p) cudaFree(p);
+        delete real;
+        delete cinner;
+    }
+};
+
+// torch.istft's NOLA check in long double: the envelope env(u) = sum_f wl[u - f * hop]^2 over the frames 0 <= f < F covering
+// the padded sample u must reach 1e-11 wherever a retained sample (u in [pad, pad + n)) is covered (u < n_fft + hop (F - 1)).
+// Between the head (u < n_fft - 1, where frame 0 clips the sum) and the tail (u >= F hop, where frame F - 1 does), env is
+// periodic in hop, so the first n_fft + hop and the last n_fft + hop retained samples hold every value it takes; scanned in
+// ascending u, the first failure found is the first there is.  Sets nola_fail to that sample (t = u - pad) or -1.
+template <typename T>
+void stft_nola(PlanStft<T>* pl, const std::vector<long double>& wl) {
+    const size_t n_fft = pl->n_fft, hop = pl->hop, F = pl->frames;
+    auto env = [&](size_t u) {
+        const size_t f_hi = std::min(u / hop, F - 1), f_lo = u >= n_fft ? (u - n_fft) / hop + 1 : 0;
+        long double s = 0;
+        for (size_t f = f_lo; f <= f_hi; ++f) s += wl[u - f * hop] * wl[u - f * hop];
+        return s;
+    };
+    const size_t lo = pl->pad, hi = std::min(pl->pad + pl->n, n_fft + hop * (F - 1)), span = n_fft + hop;
+    const size_t head_end = std::min(hi, lo + span), tail_lo = std::max(head_end, hi > span ? hi - span : 0);
+    for (size_t r = 0; r < 2; ++r)
+        for (size_t u = r ? tail_lo : lo; u < (r ? hi : head_end); ++u) {
+            const long double e = env(u);
+            if (e < 1e-11L) { pl->nola_fail = (long long)(u - lo); pl->nola_env = e; return; }
+        }
+    pl->nola_fail = -1;
+}
+
+template <typename T>
+int32_t build_plan_stft(size_t n, size_t n_fft, size_t hop, const T* window, size_t win_length, int center, int pad_mode, int domain,
+                        int device, PlanStft<T>** out) {
+    if (!out) return fail(PHASTFT_ERR_INVALID_ARG, "out == NULL");
+    *out = nullptr;
+    if (n == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n must be >= 1");
+    if (n_fft == 0) return fail(PHASTFT_ERR_INVALID_ARG, "n_fft must be >= 1");
+    if (hop == 0) return fail(PHASTFT_ERR_INVALID_ARG, "hop must be >= 1");
+    if (win_length == 0 || win_length > n_fft)
+        return fail(PHASTFT_ERR_INVALID_ARG, "win_length must be in [1, n_fft = " + std::to_string(n_fft) + "] (got " + std::to_string(win_length) + ")");
+    if (pad_mode != PHASTFT_STFT_PAD_REFLECT && pad_mode != PHASTFT_STFT_PAD_CONSTANT)
+        return fail(PHASTFT_ERR_INVALID_ARG, "pad_mode must be PHASTFT_STFT_PAD_REFLECT or PHASTFT_STFT_PAD_CONSTANT");
+    if (domain != PHASTFT_STFT_REAL && domain != PHASTFT_STFT_COMPLEX)
+        return fail(PHASTFT_ERR_INVALID_ARG, "domain must be PHASTFT_STFT_REAL or PHASTFT_STFT_COMPLEX");
+    const size_t pad = center ? n_fft / 2 : 0;
+    if (center && pad_mode == PHASTFT_STFT_PAD_REFLECT && pad >= n)
+        return fail(PHASTFT_ERR_INVALID_ARG, "reflect padding of n_fft / 2 = " + std::to_string(pad) + " needs n > " + std::to_string(pad) +
+                                             " (got n = " + std::to_string(n) + ")");
+    if (!center && n < n_fft)
+        return fail(PHASTFT_ERR_INVALID_ARG, "without centering n must be >= n_fft = " + std::to_string(n_fft) + " (got n = " + std::to_string(n) + ")");
+    const bool cplx = domain == PHASTFT_STFT_COMPLEX;
+    std::unique_ptr<PlanStft<T>> pl(new PlanStft<T>());
+    pl->n = n; pl->n_fft = n_fft; pl->hop = hop; pl->pad = pad; pl->device = device; pl->cplx = cplx;
+    pl->reflect = center && pad_mode == PHASTFT_STFT_PAD_REFLECT;
+    pl->frames = 1 + (n + 2 * pad - n_fft) / hop;
+    pl->bins = cplx ? n_fft : n_fft / 2 + 1;
+    if (int32_t st = cplx ? build_plan_any<T>(n_fft, device, PHASTFT_ANY_AUTO, &pl->cinner)
+                          : build_plan_r2c_any<T>(n_fft, device, PHASTFT_ANY_AUTO, &pl->real))
+        return st;
+    // torch's window: win_length values (ones when NULL) centred in n_fft, left offset (n_fft - win_length) / 2
+    std::vector<long double> wl(n_fft, 0.0L);
+    const size_t left = (n_fft - win_length) / 2;
+    for (size_t i = 0; i < win_length; ++i) wl[left + i] = window ? (long double)window[i] : 1.0L;
+    std::vector<T> wt(2 * n_fft);
+    const long double norm = 1.0L / sqrtl((long double)n_fft);
+    for (size_t i = 0; i < n_fft; ++i) { wt[i] = (T)wl[i]; wt[n_fft + i] = (T)(wl[i] * norm); }
+    stft_nola(pl.get(), wl);
+    DeviceGuard g(device);
+    CUDA_TRY(cudaMalloc(&pl->win, 2 * n_fft * sizeof(T)));
+    CUDA_TRY(cudaMemcpy(pl->win, wt.data(), 2 * n_fft * sizeof(T), cudaMemcpyHostToDevice));
+    if (int32_t st = pl->w.init(pl->frames * pl->member_elems())) return st;   // room for one member; batched calls grow it
+    pl->description = "n=" + std::to_string(n) + " n_fft=" + std::to_string(n_fft) + " hop=" + std::to_string(hop) +
+                      (sizeof(T) == 8 ? " f64" : " f32") + " stft " + (cplx ? "complex" : "real") + " F=" + std::to_string(pl->frames) + " | ";
+    *out = pl.release();
+    return PHASTFT_OK;
+}
+
+template <typename T>
+std::string stft_description(const PlanStft<T>* pl) {
+    return pl->description + (pl->cplx ? pl->cinner->description : r2c_any_description(pl->real));
+}
+
+// Every allocation a call of `batch` members would make: the inner plan's for batch x F frames, and the workspace.
+template <typename T>
+int32_t stft_reserve(const PlanStft<T>* pl, size_t batch) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const size_t frames = batch * pl->frames;
+    if (int32_t st = pl->cplx ? any_reserve(pl->cinner, frames) : r2c_any_reserve(pl->real, frames)) return st;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    return pl->w.grow(frames * pl->member_elems(), batch);
+}
+
+// One STFT-FRAME (over frames) or ISTFT-OLA (over members), `threads` threads per member, from member 0, in launches of at most
+// 2^31 - 1 blocks.  Launch record: R = n_fft, C = the members of that launch.
+template <typename T>
+int32_t launch_stft_stage(bool ola, bool cplx, bool even_fix, StftParams<T> p, size_t threads, size_t members, cudaStream_t stream) {
+    const size_t bpm = (threads + 255) / 256;
+    p.blocks_per_member = (unsigned)bpm;
+    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    for (size_t done = 0; done < members; done += max_members) {
+        const size_t nb = std::min(members - done, max_members);
+        p.m0 = (long long)done;
+        launch_stft<T>(ola, cplx, even_fix, p, (unsigned)(nb * bpm), stream);
+        CUDA_TRY(cudaGetLastError());
+        note_launch({ola ? "ISTFT-OLA" : "STFT-FRAME", (int)std::min<long long>(p.n_fft, INT32_MAX), 0, (int)nb, 256, 0, "plain", false});
+    }
+    return PHASTFT_OK;
+}
+
+// The arguments both directions share: `sig` the caller's signals (member b at sig + b * sig_stride values, n of them), `spec`
+// the caller's spectra (frame b * F + f at spec + (b * F + f) * frame_stride complex values, bins of them).
+template <typename T>
+int32_t stft_check(const PlanStft<T>* pl, int normalized, const T* sig, size_t sig_stride, const T* spec, size_t frame_stride,
+                   size_t batch, bool inverse) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const char* sname = inverse ? "d_y" : "d_x";
+    if (normalized != 0 && normalized != 1) return fail(PHASTFT_ERR_INVALID_ARG, "normalized must be 0 or 1");
+    if (!sig) return fail(PHASTFT_ERR_INVALID_ARG, std::string(sname) + " == NULL");
+    if (!spec) return fail(PHASTFT_ERR_INVALID_ARG, "d_spec == NULL");
+    const size_t n = pl->n, bins = pl->bins, F = pl->frames, v = pl->vals();
+    if (frame_stride < bins)
+        return fail(PHASTFT_ERR_INVALID_ARG, "frame_stride must be >= the bin count " + std::to_string(bins) + " (got " + std::to_string(frame_stride) + ")");
+    if (batch > 1 && sig_stride < n)
+        return fail(PHASTFT_ERR_INVALID_ARG, std::string(inverse ? "y_stride" : "x_stride") + " must be >= n = " + std::to_string(n) +
+                                             " (got " + std::to_string(sig_stride) + ")");
+    if (int32_t st = check_pair_alignment(spec, "d_spec")) return st;
+    if (pl->cplx)
+        if (int32_t st = check_pair_alignment(sig, sname)) return st;
+    if (batch == 0) return PHASTFT_OK;
+    const uintptr_t s0 = reinterpret_cast<uintptr_t>(sig), s1 = s0 + ((batch - 1) * sig_stride + n) * v * sizeof(T);
+    const uintptr_t p0 = reinterpret_cast<uintptr_t>(spec), p1 = p0 + ((batch * F - 1) * frame_stride + bins) * 2 * sizeof(T);
+    if (s0 < p1 && p0 < s1) return fail(PHASTFT_ERR_INVALID_ARG, std::string("d_spec's frames overlap ") + sname + "'s members");
+    return PHASTFT_OK;
+}
+
+// Member b's n values at d_x + b * x_stride (reals, or complex pairs aligned to 2 * sizeof(T)) give F frames of bins bins at
+// d_spec + (b * F + f) * frame_stride complex values; the values between frames are never written.
+template <typename T>
+int32_t stft_dev(const PlanStft<T>* pl, int normalized, const T* d_x, size_t x_stride, T* d_spec, size_t frame_stride, size_t batch,
+                 cudaStream_t stream) {
+    if (int32_t st = stft_check(pl, normalized, d_x, x_stride, d_spec, frame_stride, batch, false)) return st;
+    if (batch == 0) return PHASTFT_OK;
+    const size_t n_fft = pl->n_fft, frames = batch * pl->frames;
+    DeviceGuard g(pl->device);
+    StftParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.x = d_x; p.win = pl->win + (normalized ? n_fft : 0);
+    p.n = (long long)pl->n; p.n_fft = (long long)n_fft; p.hop = (long long)pl->hop; p.pad = (long long)pl->pad;
+    p.n_frames = (long long)pl->frames; p.x_stride = (long long)x_stride; p.reflect = pl->reflect;
+    if (pl->cplx) {   // framed straight into the caller's slots and transformed in place there
+        p.frames = d_spec; p.fstride = (long long)frame_stride;
+        int32_t st = launch_stft_stage<T>(false, true, false, p, n_fft, frames, stream);
+        if (!st) st = any_interleaved_dev(pl->cinner, d_spec, PHASTFT_FORWARD, frames, frame_stride, stream);
+        return st;
+    }
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    bool capturing = false;
+    if (int32_t st = pl->w.acquire(frames * pl->member_elems(), batch, stream, "phastft_plan_stft_*_reserve", capturing)) return st;
+    T* ws = reinterpret_cast<T*>(pl->w.ws);
+    p.frames = ws; p.fstride = (long long)pl->fstride();
+    int32_t st = launch_stft_stage<T>(false, false, false, p, n_fft, frames, stream);
+    if (!st) st = r2c_il_any_dev(pl->real, ws, pl->fstride(), d_spec, frame_stride, frames, stream);
+    const int32_t rel = pl->w.release(stream, capturing);   // also after a failed launch: the kernels queued so far used it
+    return st ? st : rel;
+}
+
+// The inverse: member b's F frames at d_spec + (b * F + f) * frame_stride (never written) give n values at d_y + b * y_stride.
+template <typename T>
+int32_t istft_dev(const PlanStft<T>* pl, int normalized, const T* d_spec, size_t frame_stride, T* d_y, size_t y_stride, size_t batch,
+                  cudaStream_t stream) {
+    if (int32_t st = stft_check(pl, normalized, d_y, y_stride, d_spec, frame_stride, batch, true)) return st;
+    if (pl->nola_fail >= 0) {
+        char env[32];
+        snprintf(env, sizeof(env), "%.3Lg", pl->nola_env);
+        return fail(PHASTFT_ERR_INVALID_ARG, "the window's overlap-add envelope is " + std::string(env) + " < 1e-11 at sample " +
+                                             std::to_string(pl->nola_fail) + " (the NOLA condition fails): the istft is not defined there");
+    }
+    if (batch == 0) return PHASTFT_OK;
+    const size_t n_fft = pl->n_fft, frames = batch * pl->frames;
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> lock(pl->w.mu);
+    bool capturing = false;
+    if (int32_t st = pl->w.acquire(frames * pl->member_elems(), batch, stream, "phastft_plan_stft_*_reserve", capturing)) return st;
+    T* ws = reinterpret_cast<T*>(pl->w.ws);
+    int32_t st = PHASTFT_OK;
+    if (pl->cplx) {
+        const size_t row = n_fft * sizeof(cx<T>);
+        if (cudaMemcpy2DAsync(ws, row, d_spec, frame_stride * sizeof(cx<T>), row, frames, cudaMemcpyDeviceToDevice, stream) != cudaSuccess) {
+            (void)cudaGetLastError();
+            st = fail(PHASTFT_ERR_CUDA, "cudaMemcpy2DAsync of the frames into the workspace failed");
+        }
+        if (!st) st = any_interleaved_dev(pl->cinner, ws, PHASTFT_REVERSE, frames, n_fft, stream);
+    } else {
+        st = c2r_il_any_dev(pl->real, d_spec, frame_stride, ws, pl->fstride(), frames, stream);
+    }
+    StftParams<T> p;
+    memset(&p, 0, sizeof(p));
+    p.frames = ws; p.fstride = (long long)pl->fstride();
+    p.spec = reinterpret_cast<const cx<T>*>(d_spec); p.spec_stride = (long long)frame_stride;
+    p.y = d_y; p.y_stride = (long long)y_stride; p.win = pl->win;
+    p.n = (long long)pl->n; p.n_fft = (long long)n_fft; p.hop = (long long)pl->hop; p.pad = (long long)pl->pad;
+    p.n_frames = (long long)pl->frames;
+    p.scale = normalized ? (T)sqrtl((long double)n_fft) : T(1);
+    p.inv_n = (T)(1.0L / (long double)n_fft);
+    const bool even_fix = !pl->cplx && n_fft % 2 == 0;
+    if (!st) st = launch_stft_stage<T>(true, pl->cplx, even_fix, p, pl->n, batch, stream);
+    const int32_t rel = pl->w.release(stream, capturing);
+    return st ? st : rel;
+}
+
+// host slices, synchronous, through one plan-owned buffer: the F x bins dense frames, then the n signal values.  Lengths in
+// values (complex ones for complex signals and for the spectrum).
+template <typename T>
+int32_t stft_stage(const PlanStft<T>* pl, cudaStream_t s) {
+    {
+        std::lock_guard<std::mutex> lock(pl->w.mu);   // released before the device call, which takes it
+        if (!pl->stage) CUDA_TRY(cudaMalloc(&pl->stage, pl->stage_elems() * sizeof(T)));
+    }
+    CUDA_TRY(scribble(pl->w.scribble_on, pl->stage, pl->stage_elems() * sizeof(T), s));
+    return PHASTFT_OK;
+}
+
+template <typename T>
+int32_t stft_host(const PlanStft<T>* pl, int normalized, const T* x, size_t len_x, T* spec, size_t len_spec) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const size_t n = pl->n, cnt = pl->frames * pl->bins, v = pl->vals();
+    if (len_x != n) return fail(PHASTFT_ERR_INPUT_LEN, "len_x " + std::to_string(len_x) + ", plan n = " + std::to_string(n));
+    if (len_spec != cnt) return fail(PHASTFT_ERR_OUTPUT_LEN, "len_spec " + std::to_string(len_spec) + ", F x bins = " + std::to_string(cnt));
+    if (!x || !spec) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->host_stream();
+    if (int32_t st = stft_stage(pl, s)) return st;
+    T* sspec = pl->stage;
+    T* sx = sspec + 2 * cnt;
+    CUDA_TRY(cudaMemcpyAsync(sx, x, n * v * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = stft_dev(pl, normalized, sx, n, sspec, pl->bins, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(spec, sspec, 2 * cnt * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
+template <typename T>
+int32_t istft_host(const PlanStft<T>* pl, int normalized, const T* spec, size_t len_spec, T* y, size_t len_y) {
+    if (!pl) return fail(PHASTFT_ERR_INVALID_ARG, "plan == NULL");
+    const size_t n = pl->n, cnt = pl->frames * pl->bins, v = pl->vals();
+    if (len_spec != cnt) return fail(PHASTFT_ERR_INPUT_LEN, "len_spec " + std::to_string(len_spec) + ", F x bins = " + std::to_string(cnt));
+    if (len_y != n) return fail(PHASTFT_ERR_OUTPUT_LEN, "len_y " + std::to_string(len_y) + ", plan n = " + std::to_string(n));
+    if (!spec || !y) return fail(PHASTFT_ERR_INVALID_ARG, "NULL slice");
+    DeviceGuard g(pl->device);
+    std::lock_guard<std::mutex> host_lock(pl->host_mu);
+    cudaStream_t s = pl->host_stream();
+    if (int32_t st = stft_stage(pl, s)) return st;
+    T* sspec = pl->stage;
+    T* sy = sspec + 2 * cnt;
+    CUDA_TRY(cudaMemcpyAsync(sspec, spec, 2 * cnt * sizeof(T), cudaMemcpyHostToDevice, s));
+    if (int32_t st = istft_dev(pl, normalized, sspec, pl->bins, sy, n, 1, s)) return st;
+    CUDA_TRY(cudaMemcpyAsync(y, sy, n * v * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    return PHASTFT_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -3938,6 +4235,8 @@ int32_t conv_host(const PlanConv<T>* pl, int op, int mode, const T* x, size_t le
 #define AS_CDCT(T, p) reinterpret_cast<const PlanDct<T>*>(p)
 #define AS_CONV(T, p) reinterpret_cast<PlanConv<T>*>(p)
 #define AS_CCONV(T, p) reinterpret_cast<const PlanConv<T>*>(p)
+#define AS_STFT(T, p) reinterpret_cast<PlanStft<T>*>(p)
+#define AS_CSTFT(T, p) reinterpret_cast<const PlanStft<T>*>(p)
 
 extern "C" {
 
@@ -4321,6 +4620,46 @@ void phastft_options_guess(size_t input_size, phastft_options* out) {
                                       const T* h, size_t len_h, T* y, size_t len_y) {                                   \
         launches_reset();                                                                                               \
         return conv_host<T>(AS_CCONV(T, p), op, mode, x, len_x, h, len_h, y, len_y);                                    \
+    }                                                                                                                   \
+    int32_t phastft_plan_stft_##SFX##_create(size_t n, size_t n_fft, size_t hop, const T* window, size_t win_length,    \
+                                             int center, int pad_mode, int domain, int device,                          \
+                                             phastft_plan_stft_##SFX** out) {                                           \
+        PlanStft<T>* pl = nullptr;                                                                                      \
+        int32_t st = build_plan_stft<T>(n, n_fft, hop, window, win_length, center, pad_mode, domain, device, &pl);     \
+        if (out) *out = reinterpret_cast<phastft_plan_stft_##SFX*>(pl);                                                 \
+        else if (pl) delete pl;                                                                                         \
+        return st;                                                                                                      \
+    }                                                                                                                   \
+    void phastft_plan_stft_##SFX##_destroy(phastft_plan_stft_##SFX* p) { delete AS_STFT(T, p); }                        \
+    size_t phastft_plan_stft_##SFX##_frames(const phastft_plan_stft_##SFX* p) { return p ? AS_CSTFT(T, p)->frames : 0; }\
+    size_t phastft_plan_stft_##SFX##_bins(const phastft_plan_stft_##SFX* p) { return p ? AS_CSTFT(T, p)->bins : 0; }    \
+    const char* phastft_plan_stft_##SFX##_describe(const phastft_plan_stft_##SFX* p) {                                  \
+        if (!p) return "";                                                                                              \
+        g_r2c_desc_text = stft_description<T>(AS_CSTFT(T, p));                                                          \
+        return g_r2c_desc_text.c_str();                                                                                 \
+    }                                                                                                                   \
+    int32_t phastft_plan_stft_##SFX##_reserve(const phastft_plan_stft_##SFX* p, size_t batch) {                         \
+        return stft_reserve<T>(AS_CSTFT(T, p), batch);                                                                  \
+    }                                                                                                                   \
+    int32_t phastft_stft_##SFX##_dev(const phastft_plan_stft_##SFX* p, int normalized, const T* x, size_t x_stride,     \
+                                     T* spec, size_t frame_stride, size_t batch, void* s) {                             \
+        launches_reset();                                                                                               \
+        return stft_dev<T>(AS_CSTFT(T, p), normalized, x, x_stride, spec, frame_stride, batch, (cudaStream_t)s);        \
+    }                                                                                                                   \
+    int32_t phastft_istft_##SFX##_dev(const phastft_plan_stft_##SFX* p, int normalized, const T* spec,                  \
+                                      size_t frame_stride, T* y, size_t y_stride, size_t batch, void* s) {              \
+        launches_reset();                                                                                               \
+        return istft_dev<T>(AS_CSTFT(T, p), normalized, spec, frame_stride, y, y_stride, batch, (cudaStream_t)s);       \
+    }                                                                                                                   \
+    int32_t phastft_stft_##SFX##_host(const phastft_plan_stft_##SFX* p, int normalized, const T* x, size_t len_x,       \
+                                      T* spec, size_t len_spec) {                                                       \
+        launches_reset();                                                                                               \
+        return stft_host<T>(AS_CSTFT(T, p), normalized, x, len_x, spec, len_spec);                                      \
+    }                                                                                                                   \
+    int32_t phastft_istft_##SFX##_host(const phastft_plan_stft_##SFX* p, int normalized, const T* spec,                 \
+                                       size_t len_spec, T* y, size_t len_y) {                                           \
+        launches_reset();                                                                                               \
+        return istft_host<T>(AS_CSTFT(T, p), normalized, spec, len_spec, y, len_y);                                     \
     }
 
 DEFINE_DIT_API(double, f64)

@@ -142,4 +142,8 @@ template <typename T> void launch_dct(bool post, int kind, const DctParams<T>& p
 enum ConvStage { CONV_STAGE_PRE = 0, CONV_STAGE_MUL = 1, CONV_STAGE_POST = 2 };
 template <typename T> void launch_conv(int stage, bool cplx, bool corr, const ConvParams<T>& p, unsigned grid, cudaStream_t stream);
 
+// defined in stft.cu: STFT-FRAME (`ola` false) or ISTFT-OLA for real or complex (`cplx`) signals, OLA with the even-n_fft c2r
+// correction (`even_fix`, real signals only)
+template <typename T> void launch_stft(bool ola, bool cplx, bool even_fix, const StftParams<T>& p, unsigned grid, cudaStream_t stream);
+
 }  // namespace phast

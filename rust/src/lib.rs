@@ -21,7 +21,7 @@ pub mod planner;
 
 use options::Options;
 use planner::{Direction, PlannerAny32, PlannerAny64, PlannerConv32, PlannerConv64, PlannerDit32, PlannerDit64, PlannerDct32, PlannerDct64,
-              PlannerR2c32, PlannerR2c64, PlannerR2cAny32, PlannerR2cAny64};
+              PlannerR2c32, PlannerR2c64, PlannerR2cAny32, PlannerR2cAny64, PlannerStft32, PlannerStft64};
 
 /// Reference panic texts by status code (include/phastft_status.h).
 #[track_caller]
@@ -391,6 +391,57 @@ impl_conv!(convolve_f32_with_planner, correlate_f32_with_planner, convolve_f32_d
            PlannerConv32, phastft_conv_f32_host, phastft_conv_f32_dev);
 
 // ------------------------------------------------------------------------------------------------
+// Additive: the short-time Fourier transform and its inverse (torch.stft / torch.istft)
+// ------------------------------------------------------------------------------------------------
+/// The safe host functions pass slice lengths in values of the slice's element type, and the library reads and writes as many
+/// values of the planner's domain, so they panic on a domain mismatch before any call (as the convolution's do).
+#[track_caller]
+fn check_stft_domain(planner_complex: bool, signal_complex: bool) {
+    if planner_complex != signal_complex {
+        panic!("PlannerStft domain mismatch: the planner was built for {} signals, the slice is {}",
+               if planner_complex { "complex" } else { "real" }, if signal_complex { "complex" } else { "real" });
+    }
+}
+macro_rules! impl_stft {
+    ($stft:ident, $istft:ident, $stft_dev:ident, $istft_dev:ident, $t:ty, $planner:ident, $host_f:ident, $host_i:ident, $dev_f:ident,
+     $dev_i:ident) => {
+        /// Real signal of a real planner: `spec` gets `frames() * bins()` interleaved (re, im) pairs as `$t` (`2 *` that
+        /// many values), frame-major.  Panics on a length mismatch, and when the planner was built for complex signals.
+        pub fn $stft(x: &[$t], spec: &mut [$t], normalized: bool, planner: &$planner) {
+            check_stft_domain(planner.is_complex(), false);
+            check(unsafe { ffi::$host_f(planner.raw, normalized as i32, x.as_ptr(), x.len(), spec.as_mut_ptr(), spec.len() / 2) });
+        }
+        /// The inverse of a real planner's frame-major spectrum into `n()` reals, with the forward form's panics.
+        pub fn $istft(spec: &[$t], y: &mut [$t], normalized: bool, planner: &$planner) {
+            check_stft_domain(planner.is_complex(), false);
+            check(unsafe { ffi::$host_i(planner.raw, normalized as i32, spec.as_ptr(), spec.len() / 2, y.as_mut_ptr(), y.len()) });
+        }
+        /// `batch` signals on device data: member b reads `n()` values at `d_x + b * x_stride` and frame f of it goes to
+        /// `d_spec + (b * frames() + f) * frame_stride` complex values, stream-ordered.
+        ///
+        /// # Safety
+        /// The pointers must be device pointers valid for the members on the planner's device, counted in values of the
+        /// planner's domain (two `$t` per value for a complex planner), `d_spec` aligned to `2 * size_of::<$t>()`.
+        pub unsafe fn $stft_dev(d_x: *const $t, x_stride: usize, d_spec: *mut $t, frame_stride: usize, normalized: bool, planner: &$planner,
+                                batch: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$dev_f(planner.raw, normalized as i32, d_x, x_stride, d_spec, frame_stride, batch, stream));
+        }
+        /// The inverse device batch: frames at `d_spec + (b * frames() + f) * frame_stride`, signals at `d_y + b * y_stride`.
+        ///
+        /// # Safety
+        /// As for the forward form.
+        pub unsafe fn $istft_dev(d_spec: *const $t, frame_stride: usize, d_y: *mut $t, y_stride: usize, normalized: bool, planner: &$planner,
+                                 batch: usize, stream: *mut std::os::raw::c_void) {
+            check(ffi::$dev_i(planner.raw, normalized as i32, d_spec, frame_stride, d_y, y_stride, batch, stream));
+        }
+    };
+}
+impl_stft!(stft_f64_with_planner, istft_f64_with_planner, stft_f64_device_batch, istft_f64_device_batch, f64, PlannerStft64,
+           phastft_stft_f64_host, phastft_istft_f64_host, phastft_stft_f64_dev, phastft_istft_f64_dev);
+impl_stft!(stft_f32_with_planner, istft_f32_with_planner, stft_f32_device_batch, istft_f32_device_batch, f32, PlannerStft32,
+           phastft_stft_f32_host, phastft_istft_f32_host, phastft_stft_f32_dev, phastft_istft_f32_dev);
+
+// ------------------------------------------------------------------------------------------------
 // r2c / c2r  (algorithms/r2c.rs:521-895)
 // ------------------------------------------------------------------------------------------------
 
@@ -601,6 +652,28 @@ mod interleaved {
     }
     impl_conv_complex!(convolve_complex_f64_with_planner, correlate_complex_f64_with_planner, f64, PlannerConv64, phastft_conv_f64_host);
     impl_conv_complex!(convolve_complex_f32_with_planner, correlate_complex_f32_with_planner, f32, PlannerConv32, phastft_conv_f32_host);
+
+    macro_rules! impl_stft_complex {
+        ($stft:ident, $istft:ident, $t:ty, $planner:ident, $host_f:ident, $host_i:ident) => {
+            /// Real or complex signal: `spec` gets `frames() * bins()` bins, frame-major.  Panics on a length mismatch, and
+            /// when the signal's domain is not the planner's.
+            pub fn $stft(x: &[Complex<$t>], spec: &mut [Complex<$t>], normalized: bool, planner: &$planner) {
+                check_stft_domain(planner.is_complex(), true);
+                check(unsafe { ffi::$host_f(planner.raw, normalized as i32, x.as_ptr() as *const $t, x.len(), spec.as_mut_ptr() as *mut $t,
+                                            spec.len()) });
+            }
+            /// The inverse of a complex planner's frame-major spectrum into `n()` complex values, with the forward form's panics.
+            pub fn $istft(spec: &[Complex<$t>], y: &mut [Complex<$t>], normalized: bool, planner: &$planner) {
+                check_stft_domain(planner.is_complex(), true);
+                check(unsafe { ffi::$host_i(planner.raw, normalized as i32, spec.as_ptr() as *const $t, spec.len(), y.as_mut_ptr() as *mut $t,
+                                            y.len()) });
+            }
+        };
+    }
+    impl_stft_complex!(stft_complex_f64_with_planner, istft_complex_f64_with_planner, f64, PlannerStft64, phastft_stft_f64_host,
+                       phastft_istft_f64_host);
+    impl_stft_complex!(stft_complex_f32_with_planner, istft_complex_f32_with_planner, f32, PlannerStft32, phastft_stft_f32_host,
+                       phastft_istft_f32_host);
 }
 #[cfg(feature = "complex-nums")]
 pub use interleaved::*;

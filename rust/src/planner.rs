@@ -305,3 +305,70 @@ impl_planner_conv!(PlannerConv64, ffi::phastft_plan_conv_f64, phastft_plan_conv_
                    phastft_plan_conv_f64_fft_len, phastft_plan_conv_f64_describe, phastft_plan_conv_f64_reserve);
 impl_planner_conv!(PlannerConv32, ffi::phastft_plan_conv_f32, phastft_plan_conv_f32_create, phastft_plan_conv_f32_destroy,
                    phastft_plan_conv_f32_fft_len, phastft_plan_conv_f32_describe, phastft_plan_conv_f32_reserve);
+
+/// The padding of `PlannerStft*` with centring: reflection (torch's default) or zeros.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+#[repr(i32)]
+pub enum StftPad {
+    Reflect = 0,
+    Constant = 1,
+}
+
+macro_rules! impl_planner_stft {
+    ($name:ident, $t:ty, $raw:ty, $create:ident, $destroy:ident, $frames:ident, $bins:ident, $describe:ident, $reserve:ident) => {
+        /// Additive: the short-time Fourier transform and its inverse (torch.stft(..., return_complex=True) /
+        /// torch.istft(..., length=n)) of signals of `n` values, real or complex, over the `n_fft`-point plan.
+        pub struct $name {
+            pub(crate) raw: *mut $raw,
+            n: usize,
+            complex: bool,
+        }
+        unsafe impl Send for $name {}
+        unsafe impl Sync for $name {}
+        impl $name {
+            /// Frames `hop` apart; `window` holds the window's values (empty: ones of `n_fft`), centred in `n_fft`;
+            /// `center` pads `n_fft / 2` values on each side with `pad`.  Panics where the library refuses the plan
+            /// (hop 0, a window longer than n_fft, reflect padding of n_fft / 2 >= n, n < n_fft without centring, ...).
+            pub fn new(n: usize, n_fft: usize, hop: usize, window: &[$t], center: bool, pad: StftPad, complex: bool) -> Self {
+                let mut raw = std::ptr::null_mut();
+                let (w, wl) = if window.is_empty() { (std::ptr::null(), n_fft) } else { (window.as_ptr(), window.len()) };
+                check(unsafe {
+                    ffi::$create(n, n_fft, hop, w, wl, center as std::os::raw::c_int, pad as std::os::raw::c_int,
+                                 complex as std::os::raw::c_int, device(), &mut raw)
+                });
+                Self { raw, n, complex }
+            }
+            pub fn n(&self) -> usize {
+                self.n
+            }
+            pub fn is_complex(&self) -> bool {
+                self.complex
+            }
+            /// F, the frames per signal.
+            pub fn frames(&self) -> usize {
+                unsafe { ffi::$frames(self.raw) }
+            }
+            /// The bins per frame: n_fft / 2 + 1 (real signals) or n_fft (complex).
+            pub fn bins(&self) -> usize {
+                unsafe { ffi::$bins(self.raw) }
+            }
+            /// `"n=<n> n_fft=<n_fft> hop=<hop> f64 stft real F=<F> | "` followed by the inner plan's describe().
+            pub fn describe(&self) -> String {
+                unsafe { std::ffi::CStr::from_ptr(ffi::$describe(self.raw)) }.to_string_lossy().into_owned()
+            }
+            /// Makes every allocation a call of `batch` signals would make, so such calls can be captured in a CUDA graph.
+            pub fn reserve(&self, batch: usize) {
+                check(unsafe { ffi::$reserve(self.raw, batch) });
+            }
+        }
+        impl Drop for $name {
+            fn drop(&mut self) {
+                unsafe { ffi::$destroy(self.raw) }
+            }
+        }
+    };
+}
+impl_planner_stft!(PlannerStft64, f64, ffi::phastft_plan_stft_f64, phastft_plan_stft_f64_create, phastft_plan_stft_f64_destroy,
+                   phastft_plan_stft_f64_frames, phastft_plan_stft_f64_bins, phastft_plan_stft_f64_describe, phastft_plan_stft_f64_reserve);
+impl_planner_stft!(PlannerStft32, f32, ffi::phastft_plan_stft_f32, phastft_plan_stft_f32_create, phastft_plan_stft_f32_destroy,
+                   phastft_plan_stft_f32_frames, phastft_plan_stft_f32_bins, phastft_plan_stft_f32_describe, phastft_plan_stft_f32_reserve);
