@@ -65,7 +65,12 @@ PHASTFT_API const char* phastft_last_launches(void);
  * calling thread's most recent execution call filled with 0xFF bytes (a NaN in f32 and f64) before using them.  Nonzero only
  * for plans built while the environment variable PHASTFT_SCRIBBLE=1 was set: such plans poison their scratch when it is
  * allocated and, with cudaMemsetAsync on the call's stream, before each call's first use, so a kernel that reads scratch it has
- * not written in the same call produces NaN.  A testing aid; it never touches constant tables and changes no result. */
+ * not written in the same call produces NaN.  A testing aid; it never touches constant tables and changes no result.
+ * A second testing aid, the environment variable PHASTFT_GRID_BLOCKS_MAX, is read on every call: the most blocks one launch of
+ * a member-major elementwise kernel (R2C-UNTANGLE*, C2R-PRE*, SMOOTH-PRE*, SMOOTH-POST-R2C*, CHIRP-*, DCT-PRE-* / DCT-POST-*,
+ * CONV-*, STFT-FRAME, ISTFT-OLA) may have.  A call whose grid would exceed it launches the kernel several times, each launch
+ * on at most max(1, cap / blocks-per-member) members, with one launch record each.  Unset, not a number, <= 0 or above
+ * 2^31 - 1 it is 2^31 - 1, gridDim.x's limit; a lower value makes those splits run at small sizes with the same results. */
 PHASTFT_API uint64_t phastft_last_scribble_bytes(void);
 /* The *_oneshot entry points (a planner per call, lib.rs:180 / r2c.rs:522,696) keep their most recent plan per
  * precision and reuse it when the next call has the same size and device; this releases those plans and their

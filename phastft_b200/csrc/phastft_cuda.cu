@@ -65,6 +65,20 @@ bool scribble_env() {
     const char* e = getenv("PHASTFT_SCRIBBLE");
     return e && atoi(e) != 0;
 }
+
+// PHASTFT_GRID_BLOCKS_MAX, read on every call: the most blocks one launch of a member-major elementwise kernel may have before
+// the call splits it into several launches (2^31 - 1, gridDim.x's limit, when unset, not a number, <= 0 or above that).  A
+// lower value makes the splits that otherwise need more than 2^31 - 1 blocks run at small sizes, so tests can reach them.
+size_t grid_blocks_max() {
+    constexpr long long limit = 0x7fffffff;
+    if (const char* e = getenv("PHASTFT_GRID_BLOCKS_MAX")) {
+        char* end = nullptr;
+        const long long v = strtoll(e, &end, 10);
+        if (end != e && *end == '\0' && v > 0 && v <= limit) return (size_t)v;
+    }
+    return (size_t)limit;
+}
+
 // before a call's first use of [p, p + bytes), ordered on `stream` (a graph node while the stream is being captured)
 cudaError_t scribble(bool on, void* p, size_t bytes, cudaStream_t stream) {
     if (!on || !p || !bytes) return cudaSuccess;
@@ -2008,7 +2022,7 @@ Tw2 r2c_tw2(const PlanR2c<T>* pl) {
 template <typename T>
 int32_t launch_real(bool untangle, const RealParams<T>& rp, size_t per, size_t members, cudaStream_t stream, bool il = false) {
     const size_t bpm = (per + 255) / 256;
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
     const size_t out_w = il && untangle ? 2 : 1, in_w = il && !untangle ? 2 : 1;   // T per bin of the interleaved side
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
@@ -2803,7 +2817,7 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
     sp.tq = (int)tq; sp.tp = (int)tp;
     sp.tiles_q = (unsigned)((Q + tq - 1) / tq);
     sp.tiles_per_member = sp.tiles_q * (unsigned)(P / tp);
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / sp.tiles_per_member);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / sp.tiles_per_member);
     for (size_t done = 0; done < batch; done += max_members) {
         const size_t nb = std::min(batch - done, max_members);
         SmoothParams<T> s2 = sp;
@@ -2840,7 +2854,7 @@ int32_t mixed_run(const Mixed<T>& mx, const T* in_re, const T* in_im, size_t in_
         pp.l = (long long)mx.n; pp.bstride = (long long)out_bstride;
         const size_t bpm = (mx.n / 2 + 1 + 255) / 256;
         pp.blocks_per_member = (unsigned)bpm;
-        const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+        const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
         for (size_t done = 0; done < batch; done += max_members) {
             const size_t nb = std::min(batch - done, max_members);
             SmoothPostParams<T> p2 = pp;
@@ -3024,7 +3038,7 @@ enum ChirpKind { CHIRP_PRE, CHIRP_MUL, CHIRP_POST };
 template <int MODE, typename T>
 int32_t launch_chirp(ChirpKind kind, const ChirpParams<T>& cp, size_t per, size_t members, cudaStream_t stream) {
     const size_t bpm = (per + 255) / 256;
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
     constexpr int PM = chirp_planar<MODE>();
     constexpr bool r2c = PM == CHIRP_R2C_HALVED || PM == CHIRP_R2C_DIRECT, c2r = PM == CHIRP_C2R_HALVED || PM == CHIRP_C2R_DIRECT;
     constexpr bool il = chirp_il<MODE>();
@@ -3632,7 +3646,7 @@ int32_t launch_dct_end(bool post, int kind, DctParams<T> p, size_t threads, size
                                              {"DCT-POST-DCT2", "DCT-POST-DCT3", "DCT-POST-DST2", "DCT-POST-DST3"}};
     const size_t bpm = (threads + 255) / 256;
     p.blocks_per_member = (unsigned)bpm;
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
     for (size_t done = 0; done < batch; done += max_members) {
         const size_t nb = std::min(batch - done, max_members);
         DctParams<T> q = p;
@@ -3818,7 +3832,7 @@ int32_t launch_conv_stage(int stage, bool cplx, bool corr, ConvParams<T> p, size
     static const char* const names[3] = {"CONV-PRE", "CONV-MUL", "CONV-POST"};
     const size_t bpm = (threads + 255) / 256;
     p.blocks_per_member = (unsigned)bpm;
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
         p.m0 = (long long)done;
@@ -4054,7 +4068,7 @@ template <typename T>
 int32_t launch_stft_stage(bool ola, bool cplx, bool even_fix, StftParams<T> p, size_t threads, size_t members, cudaStream_t stream) {
     const size_t bpm = (threads + 255) / 256;
     p.blocks_per_member = (unsigned)bpm;
-    const size_t max_members = std::max<size_t>(1, size_t(0x7fffffff) / bpm);
+    const size_t max_members = std::max<size_t>(1, grid_blocks_max() / bpm);
     for (size_t done = 0; done < members; done += max_members) {
         const size_t nb = std::min(members - done, max_members);
         p.m0 = (long long)done;
